@@ -55,6 +55,7 @@ struct Counters {
 	int t_max_lq, t_max_rl;
 	int n_many;      /* reads with more chains than the lane kernel takes (K3) */
 	u32 n_swtasks;   /* local alignments the seed-level filter of long reads asks for (K3) */
+	u64 fm_total[3]; /* fastmap: lines, suffix-array rows and text bytes of the batch (totals of the scans) */
 };
 
 struct DevBuf { void *p; size_t cap; };
@@ -134,6 +135,9 @@ struct bwag_batch {
 	DevBuf d_pre_n, d_pre_score, d_pre_cig;    /* K5L results for the warp kernel */
 	DevBuf d_sel;
 	HostBuf h_pe_is, h_cflag, h_rec, h_text, h_ptab;
+	/* fastmap (bwag_fastmap.cu) */
+	DevBuf d_fm_lbeg, d_fm_lines, d_fm_nrow, d_fm_rbeg, d_fm_rows, d_fm_tlen, d_fm_tbeg, d_fm_text, d_fm_toff;
+	HostBuf h_fm_text, h_fm_off;
 	int tail_ready;              /* bwag_tail_regs ran on this batch */
 	int regs_on_device;          /* bwag_chain_extend left the regions in HBM */
 };
@@ -221,6 +225,7 @@ static int pick_grid(bwag_ctx_t *c)
 	CK(cudaGetDeviceProperties(&prop, c->device));
 	c->n_sm = prop.multiProcessorCount;
 	CK(cudaFuncSetAttribute(k_smem, cudaFuncAttributeMaxDynamicSharedMemorySize, K1_SMEM_MAX));
+	CK(cudaFuncSetAttribute(k_smem_fm, cudaFuncAttributeMaxDynamicSharedMemorySize, K1_SMEM_MAX));
 #ifndef K1_PACKED8
 	CK(cudaFuncSetAttribute(k_smem_c, cudaFuncAttributeMaxDynamicSharedMemorySize, K1_SMEM_MAX));
 #endif
@@ -651,6 +656,8 @@ static void batch_free(bwag_batch_t *b)
 	free_dev(&b->d_pre_n); free_dev(&b->d_pre_score); free_dev(&b->d_pre_cig);
 	free_dev(&b->d_dregs); free_dev(&b->d_dreg_beg); free_dev(&b->d_dreg_n); free_dev(&b->d_task_beg); free_dev(&b->d_cflag); free_dev(&b->d_pe_is); free_dev(&b->d_rec); free_dev(&b->d_text); free_dev(&b->d_ptab);
 	free_host(&b->h_pe_is); free_host(&b->h_cflag); free_host(&b->h_rec); free_host(&b->h_text); free_host(&b->h_ptab);
+	free_dev(&b->d_fm_lbeg); free_dev(&b->d_fm_lines); free_dev(&b->d_fm_nrow); free_dev(&b->d_fm_rbeg); free_dev(&b->d_fm_rows);
+	free_dev(&b->d_fm_tlen); free_dev(&b->d_fm_tbeg); free_dev(&b->d_fm_text); free_dev(&b->d_fm_toff); free_host(&b->h_fm_text); free_host(&b->h_fm_off);
 	free(b);
 }
 
@@ -713,7 +720,12 @@ static double elapsed_at(bwag_ctx_t *c, const char *stage, int line)
 
 /* ------------------------------------------------------------------------------------------------ stage 1 */
 
-extern "C" int bwag_seed(bwag_batch_t *b, const bwag_seed_par_t *par, bwag_seeds_t *out)
+/* fastmap's form of K1 (k_smem_fm): -i and -I; NULL = the seeding of `mem` */
+struct FmK1 { int min_intv; u64 max_intv; };
+
+/* K1 (+ K1f, K1b, K2 for `mem`).  fm != NULL: K1 alone, in its fastmap form, with the same scratch sizing and repeats; the read's
+ * matches stay in HBM (b->n_intv of them in the pool) */
+static int seed_impl(bwag_batch_t *b, const bwag_seed_par_t *par, const FmK1 *fm, bwag_seeds_t *out)
 {
 	bwag_ctx_t *c = &b->lc;
 	CK(cudaSetDevice(c->device));
@@ -728,7 +740,7 @@ extern "C" int bwag_seed(bwag_batch_t *b, const bwag_seed_par_t *par, bwag_seeds
 #ifndef K1_PACKED8
 	{
 		const char *e = getenv("BWA_B200_K1_COMPACT");
-		k1c = (e ? atoi(e) != 0 : K1_COMPACT_DEFAULT) && c->ix.ktab_k > 0;
+		k1c = (e ? atoi(e) != 0 : K1_COMPACT_DEFAULT) && c->ix.ktab_k > 0 && !fm;   /* fastmap needs every match's interval (-I): k_smem */
 	}
 	/* k_smem_c checks every list and result append, so long reads start with scratch for what they typically need (a few
 	 * candidates with an interval per list, a result per ~4 bases) instead of the worst case: more lanes fit the scratch budget.
@@ -775,12 +787,14 @@ extern "C" int bwag_seed(bwag_batch_t *b, const bwag_seed_par_t *par, bwag_seeds
 			if (k1c) CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_smem_c, K1_THREADS, smem));
 			else
 #endif
+			if (fm) CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_smem_fm, K1_THREADS, smem));
+			else
 			CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_smem, K1_THREADS, smem));
 			if (cap > 0 && nb > cap) nb = cap;
 			grid = c->n_sm * (nb > 0 ? nb : 1);
 		}
 #endif
-		const int cap3 = b->max_len / (par->min_seed_len + 1) + 2;
+		const int cap3 = fm ? 1 : b->max_len / (par->min_seed_len + 1) + 2;   /* fastmap: no third pass (and -l may be -1) */
 		size_t per_group = (size_t)((k1c ? 2 : 4) * cap_list + 2 * cap_mem) * 16;   /* k_smem_c has no per-call result array */
 		{   /* keep the per-group scratch within ~6 GB: very long reads get fewer groups */
 			size_t budget = (size_t)6 << 30;
@@ -823,11 +837,15 @@ extern "C" int bwag_seed(bwag_batch_t *b, const bwag_seed_par_t *par, bwag_seeds
 		if (k1c) BWAG_LAUNCH(k_smem_c, grid, K1_THREADS, smem, c->stream, c->ix, a);
 		else
 #endif
+		if (fm) BWAG_LAUNCH(k_smem_fm, grid, K1_THREADS, smem, c->stream, c->ix, a, fm->min_intv, fm->max_intv);
+		else
 		BWAG_LAUNCH(k_smem, grid, K1_THREADS, smem, c->stream, c->ix, a);
 		CK(cudaGetLastError());
 		CK(cudaEventRecord(c->ev1, c->stream));
-		BWAG_LAUNCH(k_seed_post, (n + K1B_THREADS - 1) / K1B_THREADS, K1B_THREADS, 0, c->stream, a);   /* harmless if K1 overflowed: the run is repeated */
-		CK(cudaGetLastError());
+		if (!fm) {
+			BWAG_LAUNCH(k_seed_post, (n + K1B_THREADS - 1) / K1B_THREADS, K1B_THREADS, 0, c->stream, a);   /* harmless if K1 overflowed: the run is repeated */
+			CK(cudaGetLastError());
+		}
 		if (fetch_counters(c)) return 1;
 		c->st.ms_smem += elapsed_at(c, "smem", __LINE__); c->st.n_launch += 2;
 		if (!(c->h_cnt->flags & 41u)) break;
@@ -842,6 +860,7 @@ extern "C" int bwag_seed(bwag_batch_t *b, const bwag_seed_par_t *par, bwag_seeds
 	}
 	c->st.occ_touches += c->h_cnt->occ_touches;
 	const i64 n_intv = (i64)c->h_cnt->n_intv, n_seeds = (i64)c->h_cnt->n_seeds;
+	if (fm) { b->n_intv = n_intv; b->n_seeds = 0; b->seeded = 0; return 0; }
 	/* K2: resolve the BWT rows left in rbeg[] to suffix-array positions, in place */
 	if (n_seeds > 0) {
 		SaArgs s;
@@ -872,6 +891,89 @@ extern "C" int bwag_seed(bwag_batch_t *b, const bwag_seed_par_t *par, bwag_seeds
 	c->st.ms_d2h += elapsed_at(c, "d2h", __LINE__);
 	out->intv_beg = (const int64_t *)b->h_intv_beg.p; out->intv_n = (const int32_t *)b->h_intv_n.p; out->intv = (const bwtintv_t *)b->h_intv.p;
 	out->seed_beg = (const int64_t *)b->h_seed_beg.p; out->rbeg = (const int64_t *)b->h_rbeg.p; out->n_intv = n_intv; out->n_seeds = n_seeds;
+	return 0;
+}
+
+extern "C" int bwag_seed(bwag_batch_t *b, const bwag_seed_par_t *par, bwag_seeds_t *out) { return seed_impl(b, par, 0, out); }
+
+/* ------------------------------------------------------------------------------------------------ fastmap */
+
+static int fm_grid(const bwag_ctx_t *c, i64 n_items)
+{
+	const i64 g = (n_items + 127) / 128, cap = (i64)c->n_sm * 16;
+	return (int)(g < 1 ? 1 : g < cap ? g : cap);
+}
+
+/* K1 in its fastmap form, then F1-F3 (bwag_fastmap.cu) with K2 between them; every buffer sized from a scan's total */
+extern "C" int bwag_fastmap(bwag_batch_t *b, const bwag_fastmap_par_t *par, bwag_fastmap_t *out)
+{
+	bwag_ctx_t *c = &b->lc, *pc = b->ctx;
+	CK(cudaSetDevice(c->device));
+	if (!pc->have_ctg) return set_err("bwag_fastmap needs the contig table (bwag_ctx_set_contigs)");
+	const int n = b->n;
+	for (int r = 0; r < n; ++r)
+		if (b->h_off[r + 1] - b->h_off[r] >= (1 << 23)) return set_err("read %d of the batch has %lld bases; reads of 2^23 bases or more are not supported", r, (long long)(b->h_off[r + 1] - b->h_off[r]));
+	bwag_seed_par_t sp;
+	memset(&sp, 0, sizeof(sp));
+	sp.min_seed_len = par->min_len;
+	const FmK1 fm = { par->min_intv < 1 ? 1 : par->min_intv, par->max_intv };
+	if (seed_impl(b, &sp, &fm, 0)) return 1;
+	const i64 n_lines = b->n_intv;
+	if (buf_reserve(&b->d_fm_lbeg, 8 * ((size_t)n + 1)) || buf_reserve(&b->d_fm_toff, 8 * ((size_t)n + 1)) ||
+	    buf_reserve(&b->d_fm_lines, sizeof(bwtintv_t) * ((size_t)n_lines + 1)) || buf_reserve(&b->d_fm_nrow, 8 * ((size_t)n_lines + 1)) ||
+	    buf_reserve(&b->d_fm_rbeg, 8 * ((size_t)n_lines + 1)) || buf_reserve(&b->d_fm_tlen, 8 * ((size_t)n_lines + 1)) || buf_reserve(&b->d_fm_tbeg, 8 * ((size_t)n_lines + 1)) ||
+	    hbuf_reserve(&b->h_fm_off, 8 * ((size_t)n + 1))) return 1;
+	FmArgs f;
+	memset(&f, 0, sizeof(f));
+	f.n_reads = n; f.n_lines = n_lines; f.max_iwidth = (u64)(i64)par->max_iwidth; f.ctg = pc->tctg;
+	f.intv_beg = (const i64 *)b->d_intv_beg.p; f.intv_n = (const int *)b->d_intv_n.p; f.intv = (const bwtintv_t *)b->d_intv.p;
+	f.lbeg = (const i64 *)b->d_fm_lbeg.p; f.lines = (bwtintv_t *)b->d_fm_lines.p; f.nrow = (i64 *)b->d_fm_nrow.p; f.rbeg = (const i64 *)b->d_fm_rbeg.p;
+	f.tlen = (i64 *)b->d_fm_tlen.p; f.tbeg = (const i64 *)b->d_fm_tbeg.p; f.toff = (i64 *)b->d_fm_toff.p;
+	/* F1: read order, rows wanted per line, their scan */
+	BWAG_LAUNCH(k_fm_scan32, 1, FM_SCAN_THREADS, 0, c->stream, (const int *)b->d_intv_n.p, (i64)n, (i64 *)b->d_fm_lbeg.p, &c->d_cnt->fm_total[0]);
+	BWAG_LAUNCH(k_fm_lines, fm_grid(c, n), 128, 0, c->stream, f);
+	BWAG_LAUNCH(k_fm_scan64, 1, FM_SCAN_THREADS, 0, c->stream, (const i64 *)b->d_fm_nrow.p, n_lines, (i64 *)b->d_fm_rbeg.p, &c->d_cnt->fm_total[1]);
+	CK(cudaGetLastError());
+	if (fetch_counters(c)) return 1;
+	c->st.n_launch += 3;
+	const i64 n_rows = (i64)c->h_cnt->fm_total[1];
+	/* F2 + K2: the rows, resolved in place */
+	if (buf_reserve(&b->d_fm_rows, 8 * ((size_t)n_rows + 1))) return 1;
+	f.rows = (i64 *)b->d_fm_rows.p;
+	if (n_rows > 0) {
+		BWAG_LAUNCH(k_fm_rows, fm_grid(c, n_lines), 128, 0, c->stream, f);
+		SaArgs s;
+		s.rbeg = f.rows; s.n = n_rows; s.next = &c->d_cnt->next_seed; s.sa_touches = &c->d_cnt->sa_touches;
+		int grid = c->grid_k2;
+		const i64 need = (n_rows + K2_THREADS - 1) / K2_THREADS;
+		if (grid > need) grid = (int)need;
+		CK(cudaEventRecord(c->ev0, c->stream));
+		BWAG_LAUNCH(k_sa, grid, K2_THREADS, 0, c->stream, c->ix, s);
+		CK(cudaGetLastError());
+		CK(cudaEventRecord(c->ev1, c->stream));
+		c->st.n_launch += 2;
+	}
+	/* F3: line sizes, their scan, the text, each read's range */
+	BWAG_LAUNCH(k_fm_text, fm_grid(c, n_lines), 128, 0, c->stream, f, 0);
+	BWAG_LAUNCH(k_fm_scan64, 1, FM_SCAN_THREADS, 0, c->stream, (const i64 *)b->d_fm_tlen.p, n_lines, (i64 *)b->d_fm_tbeg.p, &c->d_cnt->fm_total[2]);
+	CK(cudaGetLastError());
+	if (fetch_counters(c)) return 1;
+	if (n_rows > 0) { c->st.ms_sa += elapsed_at(c, "sa", __LINE__); c->st.sa_touches += c->h_cnt->sa_touches; }
+	c->st.n_launch += 2;
+	const i64 n_text = (i64)c->h_cnt->fm_total[2];
+	if (buf_reserve(&b->d_fm_text, (size_t)n_text + 1) || hbuf_reserve(&b->h_fm_text, (size_t)n_text + 1)) return 1;
+	f.text = (char *)b->d_fm_text.p;
+	BWAG_LAUNCH(k_fm_text, fm_grid(c, n_lines), 128, 0, c->stream, f, 1);
+	BWAG_LAUNCH(k_fm_readoff, fm_grid(c, (i64)n + 1), 128, 0, c->stream, f);
+	CK(cudaGetLastError());
+	c->st.n_launch += 2;
+	CK(cudaEventRecord(c->ev0, c->stream));
+	if (n_text) D2H(c, b->h_fm_text.p, b->d_fm_text.p, (size_t)n_text);
+	D2H(c, b->h_fm_off.p, b->d_fm_toff.p, 8 * ((size_t)n + 1));
+	CK(cudaEventRecord(c->ev1, c->stream));
+	CK(stream_wait(c));
+	c->st.ms_d2h += elapsed_at(c, "d2h", __LINE__);
+	out->text = (const char *)b->h_fm_text.p; out->off = (const int64_t *)b->h_fm_off.p;
 	return 0;
 }
 

@@ -119,6 +119,18 @@ struct GlbLaneArgs {
 
 /* ---- stage 4 (device tail, bwag_tail.cu) ---- */
 struct TailCtg { i64 l_pac; int n_seqs; const i64 *off; const int *len; const uint8_t *alt; const char *names; const int *name_off; };   /* bntann1_t columns; names back to back, name_off[n_seqs+1] */
+__device__ __forceinline__ int t_pos2rid(const TailCtg &c, i64 pos_f)   /* bntseq.c:354-368 */
+{
+	int lo = 0, hi = c.n_seqs, mid = 0;
+	if (pos_f >= c.l_pac) return -1;
+	while (lo < hi) {
+		mid = (lo + hi) >> 1;
+		if (pos_f < c.off[mid]) hi = mid;
+		else if (mid == c.n_seqs - 1 || pos_f < c.off[mid + 1]) break;
+		else lo = mid + 1;
+	}
+	return mid;
+}
 
 struct TailRegsArgs {
 	int n_reads, pe;
@@ -158,6 +170,27 @@ struct SwArgs {
 	unsigned char *scratch; i64 per_thread; int cap_n, cap_q, cap_t;   /* per lane: 4 x short[cap_n], u64[cap_t], query[cap_q], target[cap_t] */
 	int *next_task; u32 *flags;
 };
+
+/* ---- fastmap (bwag_fastmap.cu) ---- */
+#define FM_SCAN_THREADS 1024
+struct FmArgs {
+	int n_reads; i64 n_lines;
+	u64 max_iwidth;                                   /* -w as the reference compares it: (uint64_t)(int64_t)w */
+	TailCtg ctg;
+	const i64 *intv_beg; const int *intv_n; const bwtintv_t *intv;   /* K1's pool */
+	const i64 *lbeg;                                  /* [n_reads+1] first line of each read (scan of intv_n) */
+	bwtintv_t *lines; i64 *nrow;                      /* [n_lines] the matches in read order, rows each one wants */
+	const i64 *rbeg; i64 *rows;                       /* [n_lines+1] first row of each line (scan of nrow); the rows, resolved by K2 */
+	i64 *tlen; const i64 *tbeg; char *text;           /* [n_lines] bytes per line, [n_lines+1] their scan, the text */
+	i64 *toff;                                        /* [n_reads+1] first byte of each read's text */
+};
+__global__ void k_fm_scan32(const int *in, i64 n, i64 *out, u64 *total);
+__global__ void k_fm_scan64(const i64 *in, i64 n, i64 *out, u64 *total);
+__global__ void k_fm_lines(FmArgs a);
+__global__ void k_fm_rows(FmArgs a);
+__global__ void k_fm_text(FmArgs a, int write);
+__global__ void k_fm_readoff(FmArgs a);
+__global__ void k_smem_fm(DevIndex ix, SeedArgs a, int min_intv, u64 max_intv);   /* K1 listing SMEMs as `bwa fastmap` does (bwag_smem.cu) */
 
 __global__ void k_chain_emit(ChainArgs a);
 __global__ void k_global_lane(DevIndex ix, GlbLaneArgs a);

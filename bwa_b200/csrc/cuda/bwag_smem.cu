@@ -339,12 +339,21 @@ __global__ void __launch_bounds__(128) k_pack_reads(const uint8_t *codes, const 
 	}
 }
 
-/* ------------------------------------------------------------------------------------------------ K1 */
+/* ------------------------------------------------------------------------------------------------ K1
+ * The body of k_smem, for two callers: `mem` (FM = false: the three seeding passes of mem_collect_intv) and `fastmap` (FM = true:
+ * the SMEM listing of smem_next, bwamem_extra.c:86-96, one bwt_smem1a call after the other, bwt.c:289-351).  In the fastmap form
+ *   - only the first pass runs, with min_intv = fm_min_intv (-i) instead of 1;
+ *   - -I (fm_max_intv > 0) stops the forward sweep as soon as the current interval is smaller (bwt.c:305), and the backward sweep
+ *     tests the size of bwt_smem1a's `ik` register, not the candidate's (bwt.c:330-331): ik2 keeps the last forward interval until a
+ *     match is recorded and is the last recorded match from then on (bwt.c:334), short matches included;
+ *   - the length filter is the reference's unsigned one (fastmap.c:460: -l < 0 keeps nothing);
+ *   - the read's list is the calls' matches, each call's in ascending start (CALL_DONE), calls in the order made: nothing sorts it.
+ * The FM = false instantiation (k_smem) keeps the registers, shared memory and SASS instruction count it had before. */
 #ifndef K1_MIN_BLOCKS
 #define K1_MIN_BLOCKS 5
 #endif
-__global__ void __launch_bounds__(K1_THREADS, K1_MIN_BLOCKS)
-k_smem(DevIndex ix, SeedArgs a)
+template <bool FM>
+__device__ __forceinline__ void smem_lane(const DevIndex &ix, const SeedArgs &a, int fm_min_intv, u64 fm_max_intv)
 {
 #ifdef BWAG_CUSIM
 	ulonglong2 *sl = reinterpret_cast<ulonglong2 *>(cusim_dyn_smem);
@@ -408,7 +417,7 @@ k_smem(DevIndex ix, SeedArgs a)
 #define CALL_DONE() do { \
 		for (int e_ = m1_n - 1; e_ >= 0; --e_) { \
 			Intv p_ = ld_intv(m1 + e_); \
-			if ((int)((u32)p_.info - (u32)(p_.info >> 32)) >= a.min_seed_len) { \
+			if (FM ? (u64)((u32)p_.info - (u32)(p_.info >> 32)) >= (u64)(i64)a.min_seed_len : (int)((u32)p_.info - (u32)(p_.info >> 32)) >= a.min_seed_len) { \
 				if (mem_n < a.cap_mem) { st_intv(mem + mem_n, p_.x0, p_.x1, p_.x2, p_.info); ++mem_n; } else overflow |= 8; \
 			} \
 		} \
@@ -424,8 +433,8 @@ k_smem(DevIndex ix, SeedArgs a)
 			if (st == ST_IDLE) {
 				if (pass == 0) {            /* first pass: all SMEMs (bwamem.c:147-157) */
 					while (x < len && QISN(x)) ++x;
-					if (x >= len) { pass = 1; k2 = 0; old_n = mem_n; continue; }
-					sx = x; min_intv = 1;
+					if (x >= len) { pass = FM ? 2 : 1; k2 = 0; old_n = mem_n; continue; }
+					sx = x; min_intv = FM ? fm_min_intv : 1;
 				} else if (pass == 1) {     /* second pass: re-seed inside long, rare SMEMs (bwamem.c:159-168) */
 					bool found = false;
 					while (k2 < old_n) {
@@ -485,8 +494,8 @@ k_smem(DevIndex ix, SeedArgs a)
 				continue;
 			}
 			if (st == ST_FWD) {
-				if (i < len && !QISN(i)) { e0 = ik0; e1 = ik1; e2 = ik2; need = true; back = 0; break; }
-				/* end of read or ambiguous base: keep the current interval, then turn around (bwt.c:317-326) */
+				if (i < len && !QISN(i) && !(FM && ik2 < fm_max_intv)) { e0 = ik0; e1 = ik1; e2 = ik2; need = true; back = 0; break; }
+				/* end of read, ambiguous base, or (fastmap -I) an interval small enough: keep the current interval, then turn around (bwt.c:305-326) */
 				ENT_ST(pl ^ 1, n_curr, ik0, ik1, ik2, ikend); ++n_curr;
 				TURN_AROUND();
 				continue;
@@ -504,6 +513,15 @@ k_smem(DevIndex ix, SeedArgs a)
 					continue;
 				}
 				if (j < n_prev) {
+					if (FM && ik2 < fm_max_intv) {   /* -I: no extension, the candidate is kept as if it died (bwt.c:330-336) */
+						if (n_curr == 0 && (m1_n == 0 || i + 1 < last_start)) {
+							u64 p0, p1, p2; u32 pe;
+							ENT_LD(pl, rev_first ? n_prev - 1 - j : j, p0, p1, p2, pe);
+							st_intv(m1 + m1_n, p0, p1, p2, (u64)(i + 1) << 32 | pe); ++m1_n; last_start = i + 1; ik2 = p2;
+						}
+						++j; K1_PF_RESET();
+						continue;
+					}
 #ifdef K1_PREFETCH   /* variant: the next candidate's entry is requested one step ahead, so that a list tail in global memory is not a serial round trip before the Occ load */
 					{
 						ulonglong2 v_;
@@ -569,6 +587,7 @@ k_smem(DevIndex ix, SeedArgs a)
 			if (o_x2 < (u64)min_intv) {
 				if (n_curr == 0 && (m1_n == 0 || i + 1 < last_start)) {
 					st_intv(m1 + m1_n, e0, e1, e2, (u64)(i + 1) << 32 | pend); ++m1_n; last_start = i + 1;
+					if (FM) ik2 = e2;       /* bwt.c:334: ik = *p */
 				}
 			} else if (n_curr == 0 || o_x2 != curr_last_x2) {
 				ENT_ST(pl ^ 1, n_curr, o_s, o_o, o_x2, pend); ++n_curr; curr_last_x2 = o_x2;
@@ -584,6 +603,19 @@ k_smem(DevIndex ix, SeedArgs a)
 		u32 f = __reduce_or_sync(FULL_MASK, overflow);
 		if ((threadIdx.x & 31) == 0 && f) atomicOr(a.flags, f);
 	}
+}
+
+__global__ void __launch_bounds__(K1_THREADS, K1_MIN_BLOCKS)
+k_smem(DevIndex ix, SeedArgs a)
+{
+	smem_lane<false>(ix, a, 1, 0);
+}
+
+/* fastmap: min_intv (-i, at least 1) and max_intv (-I, 0 = off); a.min_seed_len is -l */
+__global__ void __launch_bounds__(K1_THREADS, K1_MIN_BLOCKS)
+k_smem_fm(DevIndex ix, SeedArgs a, int min_intv, u64 max_intv)
+{
+	smem_lane<true>(ix, a, min_intv, max_intv);
 }
 
 #ifndef K1_PACKED8

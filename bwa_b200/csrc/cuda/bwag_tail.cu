@@ -39,18 +39,6 @@ __device__ __forceinline__ u64 t_mix64(u64 k)   /* hash_64 (utils.h:98-109) */
 	k += ~(k << 27); k ^= (k >> 31);
 	return k;
 }
-__device__ __forceinline__ int t_pos2rid(const TailCtg &c, i64 pos_f)   /* bntseq.c:354-368 */
-{
-	int lo = 0, hi = c.n_seqs, mid = 0;
-	if (pos_f >= c.l_pac) return -1;
-	while (lo < hi) {
-		mid = (lo + hi) >> 1;
-		if (pos_f < c.off[mid]) hi = mid;
-		else if (mid == c.n_seqs - 1 || pos_f < c.off[mid + 1]) break;
-		else lo = mid + 1;
-	}
-	return mid;
-}
 __device__ __forceinline__ i64 t_depos(const TailCtg &c, i64 pos, int *is_rev) { *is_rev = pos >= c.l_pac; return *is_rev ? (c.l_pac << 1) - 1 - pos : pos; }
 /* orientation class (0 FF, 1 FR, 2 RF, 3 RR) and distance of two hits (mem_infer_dir, bwamem_pair.c:48-56) */
 __device__ __forceinline__ int t_infer_dir(i64 l_pac, i64 b1, i64 b2, i64 *dist)

@@ -1,0 +1,215 @@
+/* bb_fastmap.c -- `bwa-b200 fastmap`: every SMEM of each read with its occurrence count and reference positions, byte for byte
+ * what the reference's `bwa fastmap` prints (fastmap.c:408-483), with the SMEM search, the suffix-array lookups and the EM lines
+ * on the GPU (bwag_fastmap: K1 in its fastmap form, K2, bwag_fastmap.cu).
+ *
+ * Three threads overlap: a reader parses the next batch of reads (BWA_B200_FASTMAP_CHUNK bases, kseq grammar: FASTA/FASTQ, plain or
+ * gzip, '-' for stdin), the calling thread runs the current one on the device, and a writer prints the previous one -- per read
+ * its SQ line, the device's EM lines and "//".  Batches pass through single-slot mailboxes, so output order is input order and at
+ * most four batches exist at a time.  BWA_B200_PROFILE=1 reports the busy time of each of the three and of the index load. */
+#include <unistd.h>
+#include <pthread.h>
+#include "bb_host.h"
+
+#define FM_MAX_LEN (1 << 23)   /* K1 keeps match ends in 23 bits (bwag_smem.cu) */
+
+typedef struct fm_batch {
+	int n;
+	int64_t *off;              /* [n+1] first base of each read in codes[] (and raw[]) */
+	uint8_t *codes;            /* 0..4 */
+	char *raw;                 /* the letters as read (-p only) */
+	bb_str_t names;            /* NUL-terminated, back to back */
+	int64_t *name_off;         /* [n] */
+	bwag_batch_t *dev;
+	bwag_fastmap_t res;
+} fm_batch_t;
+
+typedef struct { pthread_mutex_t mu; pthread_cond_t cv; fm_batch_t *slot; int full; } fm_mbox_t;   /* full with slot == NULL: end of input */
+static void mb_init(fm_mbox_t *m) { pthread_mutex_init(&m->mu, 0); pthread_cond_init(&m->cv, 0); m->slot = 0; m->full = 0; }
+static void mb_put(fm_mbox_t *m, fm_batch_t *b)
+{
+	pthread_mutex_lock(&m->mu);
+	while (m->full) pthread_cond_wait(&m->cv, &m->mu);
+	m->slot = b; m->full = 1;
+	pthread_cond_broadcast(&m->cv);
+	pthread_mutex_unlock(&m->mu);
+}
+static fm_batch_t *mb_get(fm_mbox_t *m)
+{
+	fm_batch_t *b;
+	pthread_mutex_lock(&m->mu);
+	while (!m->full) pthread_cond_wait(&m->cv, &m->mu);
+	b = m->slot; m->slot = 0; m->full = 0;
+	pthread_cond_broadcast(&m->cv);
+	pthread_mutex_unlock(&m->mu);
+	return b;
+}
+
+typedef struct {
+	bb_fq_t *fq;
+	int64_t chunk;
+	int print_seq;
+	fm_mbox_t to_dev, to_write;
+	double t_read, t_write;
+} fm_run_t;
+
+static void batch_free(fm_batch_t *b)
+{
+	if (!b) return;
+	if (b->dev) bwag_batch_end(b->dev);
+	free(b->off); free(b->codes); free(b->raw); free(b->names.s); free(b->name_off);
+	free(b);
+}
+
+/* the next batch: reads until chunk bases are reached (at least one read), NULL at the end of the input */
+static fm_batch_t *read_batch(fm_run_t *r)
+{
+	const bb_str_t *name, *comment, *seq;
+	fm_batch_t *b = 0;
+	int64_t m = 0, bases = 0, m_bases = 0;
+	while (bases < r->chunk || !b) {
+		int len = bb_fq_read1(r->fq, &name, &comment, &seq), i;
+		if (len < 0) break;   /* end of input, or a truncated quality string: kseq_read < 0 ends the reference's loop too */
+		if (len >= FM_MAX_LEN) bb_fatal("main_fastmap", "read '%s' has %d bases; reads of 2^23 (%d) bases or more are not supported", name->s, len, FM_MAX_LEN);
+		if (!b) { b = bb_calloc(1, sizeof(*b)); m = 1024; b->off = bb_malloc(8 * (size_t)(m + 1)); b->name_off = bb_malloc(8 * (size_t)m); b->off[0] = 0; }
+		if (b->n == m) { m <<= 1; b->off = bb_realloc(b->off, 8 * (size_t)(m + 1)); b->name_off = bb_realloc(b->name_off, 8 * (size_t)m); }
+		if (bases + len > m_bases) {
+			m_bases = m_bases ? m_bases : 1 << 16;
+			while (m_bases < bases + len) m_bases <<= 1;
+			b->codes = bb_realloc(b->codes, (size_t)m_bases);
+			if (r->print_seq) b->raw = bb_realloc(b->raw, (size_t)m_bases);
+		}
+		for (i = 0; i < len; ++i) { const int c = bb_nt4_table[(unsigned char)seq->s[i]]; b->codes[bases + i] = (uint8_t)(c > 4 ? 4 : c); }
+		if (r->print_seq && len) memcpy(b->raw + bases, seq->s, (size_t)len);
+		b->name_off[b->n] = (int64_t)b->names.l;
+		bb_putsn(&b->names, name->s, name->l);
+		bb_putc(&b->names, 0);   /* a NUL inside the text, after the name */
+		bases += len;
+		b->off[++b->n] = bases;
+	}
+	if (b && !b->codes) b->codes = bb_malloc(16);   /* a batch of empty reads */
+	return b;
+}
+
+static void *reader_main(void *arg)
+{
+	fm_run_t *r = arg;
+	for (;;) {
+		double t0 = bb_realtime();
+		fm_batch_t *b = read_batch(r);
+		r->t_read += bb_realtime() - t0;
+		mb_put(&r->to_dev, b);
+		if (!b) return 0;
+	}
+}
+
+static void write_batch(const fm_run_t *r, const fm_batch_t *b)
+{
+	bb_str_t s = {0, 0, 0};
+	int i;
+	for (i = 0; i < b->n; ++i) {
+		const int64_t len = b->off[i + 1] - b->off[i], t0 = b->res.off[i], t1 = b->res.off[i + 1];
+		bb_puts(&s, "SQ\t");
+		bb_puts(&s, b->names.s + b->name_off[i]);
+		bb_putc(&s, '\t');
+		bb_putl(&s, len);
+		if (r->print_seq) { bb_putc(&s, '\t'); bb_putsn(&s, b->raw + b->off[i], (size_t)len); }   /* err_puts: the letters as read, then a newline */
+		bb_putc(&s, '\n');
+		bb_putsn(&s, b->res.text + t0, (size_t)(t1 - t0));
+		bb_puts(&s, "//\n");
+		if (s.l >= (1 << 20)) {
+			if (fwrite(s.s, 1, s.l, stdout) != s.l) bb_fatal("main_fastmap", "fail to write the output");
+			s.l = 0;
+		}
+	}
+	if (s.l && fwrite(s.s, 1, s.l, stdout) != s.l) bb_fatal("main_fastmap", "fail to write the output");
+	free(s.s);
+}
+
+static void *writer_main(void *arg)
+{
+	fm_run_t *r = arg;
+	fm_batch_t *b;
+	while ((b = mb_get(&r->to_write)) != 0) {
+		double t0 = bb_realtime();
+		write_batch(r, b);
+		batch_free(b);   /* the device batch too: its pinned text buffer held the EM lines until now */
+		r->t_write += bb_realtime() - t0;
+	}
+	return 0;
+}
+
+static void usage(int min_len, int w, int min_intv, int max_len, uint64_t max_intv)
+{
+	fprintf(stderr, "\n");
+	fprintf(stderr, "Usage:   bwa-b200 fastmap [options] <idxbase> <in.fq>\n\n");
+	fprintf(stderr, "Options: -l INT    min SMEM length to output [%d]\n", min_len);
+	fprintf(stderr, "         -w INT    max interval size to find coordinates [%d]\n", w);
+	fprintf(stderr, "         -i INT    min SMEM interval size [%d]\n", min_intv);
+	fprintf(stderr, "         -L INT    max MEM length [%d] (accepted; no effect, as in bwa fastmap)\n", max_len);
+	fprintf(stderr, "         -I INT    stop if MEM is longer than -l with a size less than INT [%ld]\n", (long)max_intv);
+	fprintf(stderr, "         -p        print the read's sequence on its SQ line\n");
+	fprintf(stderr, "\n");
+}
+
+int bb_fastmap_main(int argc, char *argv[])
+{
+	int c, min_iwidth = 20, min_len = 17, print_seq = 0, min_intv = 1, max_len = 0x7fffffff;
+	uint64_t max_intv = 0;
+	bwaidx_t *idx;
+	bwag_ctx_t *ctx;
+	fm_run_t run;
+	bwag_fastmap_par_t par;
+	pthread_t th_r, th_w;
+	double t0, t_load, t_dev = 0;
+	const char *e;
+
+	while ((c = getopt(argc, argv, "w:l:pi:I:L:")) >= 0) {   /* fastmap.c:419-429 */
+		switch (c) {
+		case 'p': print_seq = 1; break;
+		case 'w': min_iwidth = atoi(optarg); break;
+		case 'l': min_len = atoi(optarg); break;
+		case 'i': min_intv = atoi(optarg); break;
+		case 'I': max_intv = (uint64_t)atol(optarg); break;
+		case 'L': max_len = atoi(optarg); break;   /* smem_next never reads it */
+		default: return 1;
+		}
+	}
+	if (optind + 1 >= argc) { usage(min_len, min_iwidth, min_intv, max_len, max_intv); return 1; }
+
+	memset(&run, 0, sizeof(run));
+	run.print_seq = print_seq;
+	run.chunk = (e = getenv("BWA_B200_FASTMAP_CHUNK")) != 0 && atol(e) > 0 ? atol(e) : 40000000;   /* bases per batch */
+	if ((run.fq = bb_fq_open(argv[optind + 1])) == 0) bb_fatal("main_fastmap", "fail to open file '%s'", argv[optind + 1]);
+	t0 = bb_realtime();
+	if ((idx = bb_idx_from_resident(argv[optind])) == 0 && (idx = bwa_idx_load(argv[optind], BWA_IDX_ALL)) == 0) { bb_fq_close(run.fq); return 1; }
+	ctx = bb_device_attach(idx->bwt, idx->bns, idx->pac);   /* fails here, before any output, if there is no GPU */
+	t_load = bb_realtime() - t0;
+	memset(&par, 0, sizeof(par));
+	par.min_len = min_len; par.min_intv = min_intv; par.max_intv = max_intv; par.max_iwidth = min_iwidth;
+
+	mb_init(&run.to_dev); mb_init(&run.to_write);
+	pthread_create(&th_r, 0, reader_main, &run);
+	pthread_create(&th_w, 0, writer_main, &run);
+	for (;;) {
+		fm_batch_t *b = mb_get(&run.to_dev);
+		double t1 = bb_realtime();
+		int rc;
+		if (!b) break;
+		if ((b->dev = bwag_batch_begin(ctx, b->n, b->codes, b->off)) == 0) bb_fatal("main_fastmap", "cannot start a device batch: %s", bwag_last_error());
+		rc = bwag_fastmap(b->dev, &par, &b->res);
+		if (rc == BWAG_UNSUPPORTED) { fprintf(stderr, "[E::%s] this build has no device SMEM lister\n", "main_fastmap"); exit(1); }
+		if (rc != 0) bb_fatal("main_fastmap", "device SMEM listing failed: %s", bwag_last_error());
+		t_dev += bb_realtime() - t1;
+		mb_put(&run.to_write, b);
+	}
+	mb_put(&run.to_write, 0);
+	pthread_join(th_r, 0);
+	pthread_join(th_w, 0);
+	if (fflush(stdout) != 0 || ferror(stdout)) bb_fatal("main_fastmap", "fail to write the output");
+	if (getenv("BWA_B200_PROFILE"))
+		fprintf(stderr, "[prof] fastmap: index load %.3f s; busy time of the reader %.3f s, the device %.3f s, the writer %.3f s; total %.3f s\n",
+		        t_load, run.t_read, t_dev, run.t_write, bb_realtime() - t0);
+	bb_fq_close(run.fq);
+	bwa_idx_destroy(idx);
+	return 0;
+}

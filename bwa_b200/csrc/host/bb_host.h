@@ -149,6 +149,9 @@ int bb_fq_read1(bb_fq_t *f, const bb_str_t **name, const bb_str_t **comment, con
 /* ---- `bwa-b200 index` (bb_index_build.c) ---- */
 int bb_index_main(int argc, char *argv[]);
 
+/* ---- `bwa-b200 fastmap` (bb_fastmap.c) ---- */
+int bb_fastmap_main(int argc, char *argv[]);
+
 #ifdef __cplusplus
 }
 #endif

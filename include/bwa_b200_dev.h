@@ -119,6 +119,24 @@ typedef struct {
 
 int bwag_seed(bwag_batch_t *b, const bwag_seed_par_t *par, bwag_seeds_t *out);   /* out == NULL: keep the results in HBM only */
 
+/* ---- SMEM listing of `bwa fastmap` (replaces the smem_next loop of main_fastmap, fastmap.c:443-475) ------------------------
+ * Per read: every SMEM of every bwt_smem1a call in the reference's order (bwamem_extra.c:86-96, bwt.c:289-351), those at least
+ * min_len long (compared as the reference does, unsigned: min_len < 0 lists nothing), each as its EM line of fastmap.c:457-473
+ * ("EM\tbeg\tend\tx[2]", then "\tname:+pos" for each of the x[2] occurrences if x[2] <= (uint64_t)max_iwidth, else "\t*\n";
+ * then "\n").  The SQ and "//" lines are the caller's.  Needs bwag_ctx_set_contigs (the contig names).  Reads of 2^23 bases or
+ * more are refused (bwag_last_error names the first).  BWAG_UNSUPPORTED from the CPU oracle of the tests. */
+typedef struct {
+	int min_len;             /* -l */
+	int min_intv;            /* -i (values below 1 act as 1, bwt.c:297) */
+	uint64_t max_intv;       /* -I (0: off) */
+	int max_iwidth;          /* -w */
+} bwag_fastmap_par_t;
+typedef struct {
+	const char *text;        /* the EM lines of all reads, in read order */
+	const int64_t *off;      /* [n_reads+1]: read r's lines are text[off[r], off[r+1]) */
+} bwag_fastmap_t;
+int bwag_fastmap(bwag_batch_t *b, const bwag_fastmap_par_t *par, bwag_fastmap_t *out);
+
 /* ---- stage 2: chain -> alignment regions (replaces the mem_chain2aln loop + ksw_extend2) ------ */
 typedef struct {
 	int a, b, o_del, e_del, o_ins, e_ins, w, zdrop, pen_clip5, pen_clip3;
