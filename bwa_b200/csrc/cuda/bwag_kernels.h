@@ -192,6 +192,40 @@ __global__ void k_fm_text(FmArgs a, int write);
 __global__ void k_fm_readoff(FmArgs a);
 __global__ void k_smem_fm(DevIndex ix, SeedArgs a, int min_intv, u64 max_intv);   /* K1 listing SMEMs as `bwa fastmap` does (bwag_smem.cu) */
 
+/* ---- aln (bwag_aln.cu) ---- */
+#define ALN_THREADS 128
+struct AlnNode { u64 k, l; u32 pos, cnt, id; int next; };   /* a queue entry, 32 bytes: see bwag_aln.cu */
+/* a lane's arena: bucket heads, bucket bitmap, widths of the read and of its seed (w, bid), then the nodes */
+struct AlnLayout { i64 heads, mask, ww, wb, sw, sb, nodes, bytes; };
+__host__ __device__ __forceinline__ AlnLayout aln_layout(int n_buckets, int max_len, int seed_cap, i64 cap_nodes)
+{
+	AlnLayout L;
+	i64 o = 0;
+	L.heads = o; o += (4 * (i64)n_buckets + 15) & ~(i64)15;
+	L.mask = o;  o += (8 * (i64)((n_buckets + 63) / 64) + 15) & ~(i64)15;
+	L.ww = o;    o += (8 * (i64)(max_len + 1) + 15) & ~(i64)15;
+	L.wb = o;    o += (4 * (i64)(max_len + 1) + 15) & ~(i64)15;
+	L.sw = o;    o += (8 * (i64)(seed_cap + 1) + 15) & ~(i64)15;
+	L.sb = o;    o += (4 * (i64)(seed_cap + 1) + 15) & ~(i64)15;
+	L.nodes = o; o += (i64)sizeof(AlnNode) * cap_nodes;
+	L.bytes = o;
+	return L;
+}
+struct AlnArgs {
+	const uint8_t *codes; const i64 *off;
+	bwag_aln_par_t par;
+	int n_buckets;                                    /* queue scores 0 .. n_buckets-1 */
+	const int *work; int n_work;                      /* the reads to search (NULL: 0 .. n_work-1) */
+	unsigned char *arena; i64 lane_bytes;             /* per lane: bucket heads and bitmap, widths, cap_nodes 32-byte nodes */
+	int cap_nodes, max_len, seed_cap, n_lanes;
+	int *n_aln; i64 *hit_beg;                         /* [n_reads] */
+	bwag_aln1_t *pool; i64 cap_pool; u64 *n_pool;     /* every read's hits, at hit_beg[r] */
+	int *redo; u32 *n_redo; u32 *flags;               /* reads to search again: 1 = their arena overflowed, 2 = the pool did */
+	int *next;
+};
+__global__ void k_aln(DevIndex ix, AlnArgs a);
+__global__ void k_aln_gather(int n_reads, const int *n_aln, const i64 *hit_beg, const bwag_aln1_t *pool, const i64 *off, bwag_aln1_t *out);
+
 __global__ void k_chain_emit(ChainArgs a);
 __global__ void k_global_lane(DevIndex ix, GlbLaneArgs a);
 __global__ void k_localsw(DevIndex ix, SwArgs a);

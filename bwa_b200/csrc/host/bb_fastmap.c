@@ -23,32 +23,11 @@ typedef struct fm_batch {
 	bwag_fastmap_t res;
 } fm_batch_t;
 
-typedef struct { pthread_mutex_t mu; pthread_cond_t cv; fm_batch_t *slot; int full; } fm_mbox_t;   /* full with slot == NULL: end of input */
-static void mb_init(fm_mbox_t *m) { pthread_mutex_init(&m->mu, 0); pthread_cond_init(&m->cv, 0); m->slot = 0; m->full = 0; }
-static void mb_put(fm_mbox_t *m, fm_batch_t *b)
-{
-	pthread_mutex_lock(&m->mu);
-	while (m->full) pthread_cond_wait(&m->cv, &m->mu);
-	m->slot = b; m->full = 1;
-	pthread_cond_broadcast(&m->cv);
-	pthread_mutex_unlock(&m->mu);
-}
-static fm_batch_t *mb_get(fm_mbox_t *m)
-{
-	fm_batch_t *b;
-	pthread_mutex_lock(&m->mu);
-	while (!m->full) pthread_cond_wait(&m->cv, &m->mu);
-	b = m->slot; m->slot = 0; m->full = 0;
-	pthread_cond_broadcast(&m->cv);
-	pthread_mutex_unlock(&m->mu);
-	return b;
-}
-
 typedef struct {
 	bb_fq_t *fq;
 	int64_t chunk;
 	int print_seq;
-	fm_mbox_t to_dev, to_write;
+	bb_mbox_t to_dev, to_write;
 	double t_read, t_write;
 } fm_run_t;
 
@@ -97,7 +76,7 @@ static void *reader_main(void *arg)
 		double t0 = bb_realtime();
 		fm_batch_t *b = read_batch(r);
 		r->t_read += bb_realtime() - t0;
-		mb_put(&r->to_dev, b);
+		bb_mbox_put(&r->to_dev, b);
 		if (!b) return 0;
 	}
 }
@@ -129,7 +108,7 @@ static void *writer_main(void *arg)
 {
 	fm_run_t *r = arg;
 	fm_batch_t *b;
-	while ((b = mb_get(&r->to_write)) != 0) {
+	while ((b = bb_mbox_get(&r->to_write)) != 0) {
 		double t0 = bb_realtime();
 		write_batch(r, b);
 		batch_free(b);   /* the device batch too: its pinned text buffer held the EM lines until now */
@@ -187,11 +166,11 @@ int bb_fastmap_main(int argc, char *argv[])
 	memset(&par, 0, sizeof(par));
 	par.min_len = min_len; par.min_intv = min_intv; par.max_intv = max_intv; par.max_iwidth = min_iwidth;
 
-	mb_init(&run.to_dev); mb_init(&run.to_write);
+	bb_mbox_init(&run.to_dev); bb_mbox_init(&run.to_write);
 	pthread_create(&th_r, 0, reader_main, &run);
 	pthread_create(&th_w, 0, writer_main, &run);
 	for (;;) {
-		fm_batch_t *b = mb_get(&run.to_dev);
+		fm_batch_t *b = bb_mbox_get(&run.to_dev);
 		double t1 = bb_realtime();
 		int rc;
 		if (!b) break;
@@ -200,9 +179,9 @@ int bb_fastmap_main(int argc, char *argv[])
 		if (rc == BWAG_UNSUPPORTED) { fprintf(stderr, "[E::%s] this build has no device SMEM lister\n", "main_fastmap"); exit(1); }
 		if (rc != 0) bb_fatal("main_fastmap", "device SMEM listing failed: %s", bwag_last_error());
 		t_dev += bb_realtime() - t1;
-		mb_put(&run.to_write, b);
+		bb_mbox_put(&run.to_write, b);
 	}
-	mb_put(&run.to_write, 0);
+	bb_mbox_put(&run.to_write, 0);
 	pthread_join(th_r, 0);
 	pthread_join(th_w, 0);
 	if (fflush(stdout) != 0 || ferror(stdout)) bb_fatal("main_fastmap", "fail to write the output");

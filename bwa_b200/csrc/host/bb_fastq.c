@@ -167,6 +167,7 @@ int bb_fq_read1(bb_fq_t *f, const bb_str_t **name, const bb_str_t **comment, con
 	*name = &f->name; *comment = &f->comment; *seq = &f->seq;
 	return r;
 }
+const bb_str_t *bb_fq_qual(const bb_fq_t *f) { return &f->qual; }   /* the quality string of the record bb_fq_read1 returned last (empty for FASTA) */
 
 static char *dup_str(const bb_str_t *s, int dup_empty)
 {

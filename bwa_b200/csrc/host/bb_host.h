@@ -145,12 +145,16 @@ bb_fq_t *bb_fq_open(const char *fn);
 bb_fq_t *bb_fq_open_range(const char *fn, int64_t beg, int64_t end);
 void bb_fq_close(bb_fq_t *f);
 int bb_fq_read1(bb_fq_t *f, const bb_str_t **name, const bb_str_t **comment, const bb_str_t **seq);
+const bb_str_t *bb_fq_qual(const bb_fq_t *f);
 
 /* ---- `bwa-b200 index` (bb_index_build.c) ---- */
 int bb_index_main(int argc, char *argv[]);
 
 /* ---- `bwa-b200 fastmap` (bb_fastmap.c) ---- */
 int bb_fastmap_main(int argc, char *argv[]);
+
+/* ---- `bwa-b200 aln` (bb_aln.c) ---- */
+int bb_aln_main(int argc, char *argv[]);
 
 #ifdef __cplusplus
 }

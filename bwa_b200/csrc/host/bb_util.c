@@ -218,3 +218,23 @@ void bb_parallel_for_lane(int lane, int nt, void (*fn)(void *, long, int), void 
 	for (pp = &g_pool.jobs; *pp; pp = &(*pp)->link) if (*pp == &job) { *pp = job.link; break; }
 	pthread_mutex_unlock(&g_pool.mu);
 }
+
+void bb_mbox_init(bb_mbox_t *m) { pthread_mutex_init(&m->mu, 0); pthread_cond_init(&m->cv, 0); m->slot = 0; m->full = 0; }
+void bb_mbox_put(bb_mbox_t *m, void *item)
+{
+	pthread_mutex_lock(&m->mu);
+	while (m->full) pthread_cond_wait(&m->cv, &m->mu);
+	m->slot = item; m->full = 1;
+	pthread_cond_broadcast(&m->cv);
+	pthread_mutex_unlock(&m->mu);
+}
+void *bb_mbox_get(bb_mbox_t *m)
+{
+	void *item;
+	pthread_mutex_lock(&m->mu);
+	while (!m->full) pthread_cond_wait(&m->cv, &m->mu);
+	item = m->slot; m->slot = 0; m->full = 0;
+	pthread_cond_broadcast(&m->cv);
+	pthread_mutex_unlock(&m->mu);
+	return item;
+}

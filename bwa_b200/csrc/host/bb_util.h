@@ -7,6 +7,7 @@
 #include <stdlib.h>
 #include <string.h>
 #include <stdio.h>
+#include <pthread.h>
 
 #ifdef __cplusplus
 extern "C" {
@@ -47,6 +48,14 @@ int bb_effective_cpus(void);   /* affinity mask capped by a cgroup CPU quota */
 int bb_parallel_ids(void);
 void bb_parallel_name(void (*fn)(void *, long, int), const char *name);   /* label a loop body for BWA_B200_PROFILE */
 void bb_parallel_report(void);   /* upper bound (exclusive) of the thread ids passed to loop bodies */
+
+/* single-slot mailbox between two threads: put waits while the slot is full, get while it is empty; the item NULL is a valid
+ * message (the commands use it for the end of the input).  Stages connected by such mailboxes keep their order and at most one
+ * item waits between two of them. */
+typedef struct { pthread_mutex_t mu; pthread_cond_t cv; void *slot; int full; } bb_mbox_t;
+void bb_mbox_init(bb_mbox_t *m);
+void bb_mbox_put(bb_mbox_t *m, void *item);
+void *bb_mbox_get(bb_mbox_t *m);
 
 typedef struct { uint64_t x, y; } bb_pair64_t;
 void bb_sort_u64(size_t n, uint64_t *a);         /* == ks_introsort_64 */

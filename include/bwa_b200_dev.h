@@ -137,6 +137,33 @@ typedef struct {
 } bwag_fastmap_t;
 int bwag_fastmap(bwag_batch_t *b, const bwag_fastmap_par_t *par, bwag_fastmap_t *out);
 
+/* ---- BWA-backtrack search of `bwa aln` (replaces bwa_cal_sa_reg_gap + bwt_match_gap, bwtaln.c:83-126, bwtgap.c:109-264) -------
+ * The batch's codes are the searched bases of each read in input order (after barcode removal and quality trimming).  Per read:
+ * the widths of the reversed read (and of its seed), then the bounded-difference backtracking search with the reference's
+ * priority queue, top-2 stop, duplicate check and width shadowing; its hits in the order the reference appends them.  Reads of
+ * 65536 bases or more are refused.  BWAG_UNSUPPORTED from the CPU oracle of the tests. */
+#define BWAG_ALN_GAPE    0x01   /* the mode bits of gap_opt_t that the search reads (bwtaln.h:94-98) */
+#define BWAG_ALN_LOGGAP  0x04
+#define BWAG_ALN_NONSTOP 0x10
+typedef struct {
+	int s_mm, s_gapo, s_gape;    /* -M -O -E (non-negative) */
+	int mode;                    /* BWAG_ALN_* bits */
+	int indel_end_skip, max_del_occ, max_entries;   /* -i -d -m */
+	int max_gapo;                /* -o clamped to the max_diff of the longest read of the reference's 262144-read group (bwtaln.c:91-94) */
+	int max_gape, max_seed_diff, seed_len, max_top2;   /* -e -k -l -R */
+	const int8_t *max_diff;      /* [n_reads] -n, or bwa_cal_maxdiff of the read's length (host libm) */
+} bwag_aln_par_t;
+/* one hit in the .sai layout (bwt_aln1_t on x86-64, bwtaln.h:43-46): bits = n_mm | n_gapo << 8 | n_gape << 16 | score << 24 |
+ * n_ins << 44 | n_del << 54, then the suffix-array interval [k, l] */
+typedef struct { uint64_t bits, k, l; } bwag_aln1_t;
+typedef struct {
+	const int32_t *n_aln;        /* [n_reads] */
+	const int64_t *off;          /* [n_reads+1]: read r's hits are aln[off[r], off[r+1]) */
+	const bwag_aln1_t *aln;
+	int64_t n_tier2;             /* reads whose queue outgrew the small per-lane arena and were searched again with a large one */
+} bwag_aln_t;
+int bwag_aln(bwag_batch_t *b, const bwag_aln_par_t *par, bwag_aln_t *out);
+
 /* ---- stage 2: chain -> alignment regions (replaces the mem_chain2aln loop + ksw_extend2) ------ */
 typedef struct {
 	int a, b, o_del, e_del, o_ins, e_ins, w, zdrop, pen_clip5, pen_clip3;
