@@ -59,6 +59,8 @@ struct Counters {
 	int aln_next;    /* aln: next read of the work list, reads listed for another run, why (1 arena, 2 pool), hits reserved in the pool, hits in all */
 	u32 aln_redo, aln_flags;
 	u64 aln_pool, aln_total;
+	u64 se_total, se_run, se_cells;   /* samse: text bytes of the batch (scan total), global alignments run and their cells */
+	int se_next, se_past;             /* samse: next refinement task; n_reads - the first read whose window runs past the forward strand (0: none) */
 };
 
 struct DevBuf { void *p; size_t cap; };
@@ -107,6 +109,8 @@ struct bwag_ctx {
 	struct bwag_ctx *parent;     /* set in the per-batch view of the context */
 	/* stage 4: contig table (offsets, lengths, ALT flags, names) and log(i) table, resident once per context */
 	void *d_tail; TailCtg tctg; const double *d_logtab; int have_ctg;
+	/* samse: the reference's holes (bns->ambs), for bns_cnt_ambi */
+	void *d_ambs; int n_holes, have_ambs;
 };
 
 struct bwag_batch {
@@ -144,6 +148,9 @@ struct bwag_batch {
 	/* aln (bwag_aln.cu) */
 	DevBuf d_aln_md, d_aln_n, d_aln_beg, d_aln_pool, d_aln_redo[2], d_aln_off, d_aln_out, d_aln_arena;
 	HostBuf h_aln_n, h_aln_off, h_aln_out;
+	/* samse (bwag_samse.cu) */
+	DevBuf d_se_reads, d_se_multi, d_se_bc, d_se_rows, d_se_pos, d_se_mpos, d_se_flags, d_se_tasks, d_se_mtask, d_se_cig, d_se_ncig, d_se_scratch, d_se_tlen, d_se_tbeg, d_se_rec, d_se_text, d_se_nm;
+	HostBuf h_se_tasks, h_se_mtask, h_se_rec, h_se_text;
 	int tail_ready;             /* bwag_tail_regs ran on this batch */
 	int regs_on_device;          /* bwag_chain_extend left the regions in HBM */
 };
@@ -445,6 +452,7 @@ extern "C" void bwag_ctx_destroy(bwag_ctx_t *c)
 		if (c->own_blob && c->blob) cudaFree(c->blob);
 	}
 	if (c->d_tail) cudaFree(c->d_tail);
+	if (c->d_ambs) cudaFree(c->d_ambs);
 	cudaFree(c->d_cnt); cudaFreeHost(c->h_cnt);
 	cudaEventDestroy(c->ev0); cudaEventDestroy(c->ev1); cudaEventDestroy(c->ev_wait);
 	cudaStreamDestroy(c->stream);
@@ -666,6 +674,9 @@ static void batch_free(bwag_batch_t *b)
 	free_dev(&b->d_fm_tlen); free_dev(&b->d_fm_tbeg); free_dev(&b->d_fm_text); free_dev(&b->d_fm_toff); free_host(&b->h_fm_text); free_host(&b->h_fm_off);
 	free_dev(&b->d_aln_md); free_dev(&b->d_aln_n); free_dev(&b->d_aln_beg); free_dev(&b->d_aln_pool); free_dev(&b->d_aln_redo[0]); free_dev(&b->d_aln_redo[1]);
 	free_dev(&b->d_aln_off); free_dev(&b->d_aln_out); free_dev(&b->d_aln_arena); free_host(&b->h_aln_n); free_host(&b->h_aln_off); free_host(&b->h_aln_out);
+	free_dev(&b->d_se_reads); free_dev(&b->d_se_multi); free_dev(&b->d_se_bc); free_dev(&b->d_se_rows); free_dev(&b->d_se_pos); free_dev(&b->d_se_mpos); free_dev(&b->d_se_flags);
+	free_dev(&b->d_se_tasks); free_dev(&b->d_se_mtask); free_dev(&b->d_se_cig); free_dev(&b->d_se_ncig); free_dev(&b->d_se_scratch); free_dev(&b->d_se_tlen); free_dev(&b->d_se_tbeg);
+	free_dev(&b->d_se_rec); free_dev(&b->d_se_text); free_dev(&b->d_se_nm); free_host(&b->h_se_tasks); free_host(&b->h_se_mtask); free_host(&b->h_se_rec); free_host(&b->h_se_text);
 	free(b);
 }
 
@@ -1108,6 +1119,167 @@ extern "C" int bwag_aln(bwag_batch_t *b, const bwag_aln_par_t *par, bwag_aln_t *
 	if (total) D2H(c, b->h_aln_out.p, b->d_aln_out.p, sizeof(bwag_aln1_t) * (size_t)total);
 	CK(stream_wait(c));
 	out->n_aln = (const int32_t *)b->h_aln_n.p; out->off = (const int64_t *)b->h_aln_off.p; out->aln = (const bwag_aln1_t *)b->h_aln_out.p;
+	return 0;
+}
+
+/* ------------------------------------------------------------------------------------------------ samse */
+
+extern "C" int bwag_ctx_set_ambs(bwag_ctx_t *c, int n_holes, const int64_t *offset, const int32_t *len)
+{
+	CK(cudaSetDevice(c->device));
+	const size_t bytes = 12 * (size_t)(n_holes > 0 ? n_holes : 0) + 16;   /* offsets | lengths */
+	char *h = (char *)calloc(1, bytes);
+	if (!h) return set_err("out of memory");
+	if (n_holes > 0) { memcpy(h, offset, 8 * (size_t)n_holes); memcpy(h + 8 * (size_t)n_holes, len, 4 * (size_t)n_holes); }
+	pthread_mutex_lock(&c->mu);
+	if (c->d_ambs) { cudaStreamSynchronize(c->stream); cudaFree(c->d_ambs); c->d_ambs = 0; c->have_ambs = 0; }
+	cudaError_t e = cudaMalloc(&c->d_ambs, bytes);
+	if (e == cudaSuccess) e = cudaMemcpy(c->d_ambs, h, bytes, cudaMemcpyHostToDevice);
+	free(h);
+	if (e != cudaSuccess) { pthread_mutex_unlock(&c->mu); return set_err("upload of the holes failed: %s", cudaGetErrorString(e)); }
+	c->n_holes = n_holes > 0 ? n_holes : 0; c->have_ambs = 1;
+	pthread_mutex_unlock(&c->mu);
+	return 0;
+}
+
+#ifdef BWAG_CUSIM
+#define SE_BUDGET ((i64)256 << 20)
+#define SE_WARPS_PER_SM 1
+#else
+#define SE_BUDGET ((i64)4 << 30)     /* per-warp scratch of the refinement (backtrack bytes above all) */
+#define SE_WARPS_PER_SM 32
+#endif
+
+/* S1, K2, S2 and S3 (bwag_samse.cu), then S4 twice around a scan: every buffer is sized from the parameters or a scan's total.
+ * The gapped hits and the room of their CIGARs are listed here, from what the caller gives (len + rlen + 2 words each: a global
+ * alignment has at most len + rlen operations); the device skips those whose hit turns out unmapped or leaves XA. */
+extern "C" int bwag_samse(bwag_batch_t *b, const bwag_samse_par_t *par, bwag_sam_t *out, int *past_end, int64_t *n_sa, int64_t *n_glb)
+{
+	bwag_ctx_t *c = &b->lc, *pc = b->ctx;
+	CK(cudaSetDevice(c->device));
+	memset(out, 0, sizeof(*out));
+	*past_end = -1; *n_sa = 0; *n_glb = 0;
+	if (!pc->have_ctg || !pc->have_ambs) return set_err("bwag_samse needs the contig table and the holes (bwag_ctx_set_contigs, bwag_ctx_set_ambs)");
+	const int n = b->n;
+	const i64 nm = par->n_multi, n_rows = (i64)n + nm;
+	if (hbuf_reserve(&b->h_se_tasks, sizeof(SeTask) * ((size_t)n_rows + 1)) || hbuf_reserve(&b->h_se_mtask, 4 * ((size_t)n_rows + 1))) return 1;
+	SeTask *tasks = (SeTask *)b->h_se_tasks.p;
+	int *mtask = (int *)b->h_se_mtask.p;   /* [n] the chosen hit's task, then [nm] each candidate's */
+	int n_tasks = 0, cap_q = 1, cap_r = 1;
+	i64 n_cig = 0, cap_z = 1, n_mapped = 0;
+	for (int r = 0; r < n; ++r) {
+		const bwag_se_read_t &p = par->reads[r];
+		if (p.len < 1 || p.len > (int)(b->h_off[r + 1] - b->h_off[r])) return set_err("read %d of the batch: %d bases searched of %lld", r, p.len, (long long)(b->h_off[r + 1] - b->h_off[r]));
+		n_mapped += p.type != 0;
+		for (int k = -1; k < p.n_multi; ++k) {
+			const i64 slot = k < 0 ? -1 : p.multi_beg + k;
+			int &mt = k < 0 ? mtask[r] : mtask[n + slot];
+			mt = -1;
+			if (k < 0 ? !(p.type && p.n_gapo) : !par->multi[slot].gap) continue;
+			const int rlen = p.len + (k < 0 ? p.ref_shift : par->multi[slot].ref_shift);
+			if (rlen < 0) return set_err("read %d of the batch: a gapped hit with %d reference bases", r, rlen);
+			int w = (int)(abs(rlen - p.len) * 1.5);
+			w = w > 50 ? w : 50;
+			const i64 n_col = p.len < 2 * w + 1 ? p.len : 2 * w + 1;
+			mt = n_tasks;
+			tasks[n_tasks].read = r; tasks[n_tasks].slot = (int)slot; tasks[n_tasks].cig_off = n_cig;
+			++n_tasks;
+			n_cig += (i64)p.len + rlen + 2;
+			if (p.len > cap_q) cap_q = p.len;
+			if (rlen > cap_r) cap_r = rlen;
+			if (n_col * rlen > cap_z) cap_z = n_col * rlen;
+		}
+	}
+	*n_sa = n_mapped + nm;
+	const size_t l_rg = par->rg_id ? strlen(par->rg_id) : 0;
+	if (buf_reserve(&b->d_se_reads, sizeof(bwag_se_read_t) * ((size_t)n + 1)) || buf_reserve(&b->d_se_multi, sizeof(bwag_se_hit_t) * ((size_t)nm + 1)) ||
+	    buf_reserve(&b->d_se_bc, (size_t)par->l_bc + l_rg + 16) || buf_reserve(&b->d_se_rows, 8 * ((size_t)n_rows + 1)) ||
+	    buf_reserve(&b->d_se_pos, 8 * ((size_t)n + 1)) || buf_reserve(&b->d_se_mpos, 8 * ((size_t)nm + 1)) || buf_reserve(&b->d_se_flags, 2 * (size_t)n_rows + 16) ||
+	    buf_reserve(&b->d_se_tasks, sizeof(SeTask) * ((size_t)n_tasks + 1)) || buf_reserve(&b->d_se_mtask, 4 * ((size_t)n_rows + 1)) ||
+	    buf_reserve(&b->d_se_cig, 4 * ((size_t)n_cig + 1)) || buf_reserve(&b->d_se_ncig, 8 * ((size_t)n_tasks + 1)) ||
+	    buf_reserve(&b->d_se_tlen, 8 * ((size_t)n + 1)) || buf_reserve(&b->d_se_tbeg, 8 * ((size_t)n + 1)) || buf_reserve(&b->d_se_nm, 4 * ((size_t)n + 1)) || buf_reserve(&b->d_se_rec, sizeof(bwag_samrec_t) * ((size_t)n + 1)) ||
+	    hbuf_reserve(&b->h_se_rec, sizeof(bwag_samrec_t) * ((size_t)n + 1))) return 1;
+	SeArgs a;
+	memset(&a, 0, sizeof(a));
+	a.n_reads = n; a.n_multi = nm; a.n_tasks = n_tasks; a.mode = par->mode; a.max_top2 = par->max_top2;
+	a.ctg = pc->tctg; a.n_holes = pc->n_holes; a.amb_off = (const i64 *)pc->d_ambs; a.amb_len = (const int *)((const char *)pc->d_ambs + 8 * (size_t)pc->n_holes);
+	a.codes = (const uint8_t *)b->d_codes.p; a.off = (const i64 *)b->d_off.p;
+	a.reads = (const bwag_se_read_t *)b->d_se_reads.p; a.multi = (const bwag_se_hit_t *)b->d_se_multi.p;
+	a.bc = (const char *)b->d_se_bc.p; a.rg = (const char *)b->d_se_bc.p + par->l_bc; a.l_rg = (int)l_rg;
+	a.rows = (i64 *)b->d_se_rows.p; a.pos = (i64 *)b->d_se_pos.p; a.mpos = (i64 *)b->d_se_mpos.p;
+	a.strand = (uint8_t *)b->d_se_flags.p; a.mapped = a.strand + n; a.mstrand = a.mapped + n; a.mkeep = a.mstrand + nm;
+	a.tasks = (const SeTask *)b->d_se_tasks.p; a.main_task = (const int *)b->d_se_mtask.p; a.multi_task = a.main_task + n;
+	a.cig = (u32 *)b->d_se_cig.p; a.ncig = (int *)b->d_se_ncig.p; a.tshift = a.ncig + n_tasks;
+	a.next_task = &c->d_cnt->se_next; a.past_end = &c->d_cnt->se_past; a.n_run = &c->d_cnt->se_run; a.cells = &c->d_cnt->se_cells;
+	a.tlen = (i64 *)b->d_se_tlen.p; a.tbeg = (const i64 *)b->d_se_tbeg.p; a.rec = (bwag_samrec_t *)b->d_se_rec.p; a.nm = (int *)b->d_se_nm.p;
+	if (reset_counters(c)) return 1;
+	if (n) H2D(c, b->d_se_reads.p, par->reads, sizeof(bwag_se_read_t) * (size_t)n);
+	if (nm) H2D(c, b->d_se_multi.p, par->multi, sizeof(bwag_se_hit_t) * (size_t)nm);
+	if (par->l_bc) H2D(c, b->d_se_bc.p, par->bc, (size_t)par->l_bc);
+	if (l_rg) H2D(c, (char *)b->d_se_bc.p + par->l_bc, par->rg_id, l_rg);
+	if (n_tasks) H2D(c, b->d_se_tasks.p, tasks, sizeof(SeTask) * (size_t)n_tasks);
+	if (n_rows) H2D(c, b->d_se_mtask.p, mtask, 4 * (size_t)n_rows);
+	/* S1 + K2: the rows, resolved in place; S2 */
+	if (n_rows) {
+		BWAG_LAUNCH(k_se_rows, fm_grid(c, n_rows), 128, 0, c->stream, a);
+		SaArgs sa;
+		sa.rbeg = a.rows; sa.n = n_rows; sa.next = &c->d_cnt->next_seed; sa.sa_touches = &c->d_cnt->sa_touches;
+		int grid = c->grid_k2;
+		const i64 need = (n_rows + K2_THREADS - 1) / K2_THREADS;
+		if (grid > need) grid = (int)need;
+		CK(cudaEventRecord(c->ev0, c->stream));
+		BWAG_LAUNCH(k_sa, grid, K2_THREADS, 0, c->stream, c->ix, sa);
+		CK(cudaEventRecord(c->ev1, c->stream));
+		BWAG_LAUNCH(k_se_pos, fm_grid(c, n), 128, 0, c->stream, a);
+		CK(cudaGetLastError());
+		c->st.n_launch += 3;
+	}
+	/* S3: persistent warps over the gapped hits, as many as the scratch budget allows */
+	if (n_tasks) {
+		const i64 per_warp = (8 * ((i64)cap_q + 2) + cap_r + cap_q + cap_z + 15) & ~(i64)15;
+		i64 warps = (i64)c->n_sm * SE_WARPS_PER_SM;
+		if (warps > n_tasks) warps = n_tasks;
+		if (warps > SE_BUDGET / per_warp) warps = SE_BUDGET / per_warp;
+		if (warps < 1) warps = 1;
+		warps = (warps + 3) & ~(i64)3;   /* whole blocks of SE_THREADS */
+		if (buf_reserve(&b->d_se_scratch, (size_t)(warps * per_warp))) return 1;
+		unsigned char *sc = (unsigned char *)b->d_se_scratch.p;
+		a.eh = (int *)sc; sc += warps * 8 * ((i64)cap_q + 2);
+		a.rseq = sc; sc += warps * (i64)cap_r;
+		a.qseq = sc; sc += warps * (i64)cap_q;
+		a.z = sc;
+		a.cap_q = cap_q; a.cap_r = cap_r; a.cap_z = cap_z;
+		CK(cudaMemsetAsync(b->d_se_ncig.p, 0, 8 * (size_t)n_tasks, c->stream));
+		BWAG_LAUNCH(k_se_refine, (int)(warps * 32 / SE_THREADS), SE_THREADS, 0, c->stream, c->ix, a);
+		CK(cudaGetLastError());
+		++c->st.n_launch;
+	}
+	/* S4: sizes, their scan, then the text */
+	if (n) BWAG_LAUNCH(k_se_text, fm_grid(c, n), 128, 0, c->stream, c->ix, a, 0);
+	BWAG_LAUNCH(k_fm_scan64, 1, FM_SCAN_THREADS, 0, c->stream, (const i64 *)b->d_se_tlen.p, (i64)n, (i64 *)b->d_se_tbeg.p, &c->d_cnt->se_total);
+	CK(cudaGetLastError());
+	if (fetch_counters(c)) return 1;
+	c->st.n_launch += 2;
+	if (n_rows) { c->st.ms_sa += elapsed_at(c, "sa", __LINE__); c->st.sa_touches += c->h_cnt->sa_touches; }
+	c->st.glb_cells += c->h_cnt->se_cells;
+	*n_glb = (int64_t)c->h_cnt->se_run;
+	if (c->h_cnt->se_past) {
+		*past_end = n - c->h_cnt->se_past;
+		return set_err("read %d of the batch: its gapped alignment window runs past the end of the forward strand", *past_end);
+	}
+	const i64 n_text = (i64)c->h_cnt->se_total;
+	if (buf_reserve(&b->d_se_text, (size_t)n_text + 1) || hbuf_reserve(&b->h_se_text, (size_t)n_text + 1)) return 1;
+	a.text = (char *)b->d_se_text.p;
+	if (n) BWAG_LAUNCH(k_se_text, fm_grid(c, n), 128, 0, c->stream, c->ix, a, 1);
+	CK(cudaGetLastError());
+	++c->st.n_launch;
+	CK(cudaEventRecord(c->ev0, c->stream));
+	if (n_text) D2H(c, b->h_se_text.p, b->d_se_text.p, (size_t)n_text);
+	if (n) D2H(c, b->h_se_rec.p, b->d_se_rec.p, sizeof(bwag_samrec_t) * (size_t)n);
+	CK(cudaEventRecord(c->ev1, c->stream));
+	CK(stream_wait(c));
+	c->st.ms_d2h += elapsed_at(c, "d2h", __LINE__);
+	out->rec = (const bwag_samrec_t *)b->h_se_rec.p; out->text = (const char *)b->h_se_text.p; out->n_text = n_text;
 	return 0;
 }
 

@@ -226,6 +226,30 @@ struct AlnArgs {
 __global__ void k_aln(DevIndex ix, AlnArgs a);
 __global__ void k_aln_gather(int n_reads, const int *n_aln, const i64 *hit_beg, const bwag_aln1_t *pool, const i64 *off, bwag_aln1_t *out);
 
+/* ---- samse (bwag_samse.cu) ---- */
+#define SE_THREADS 128
+struct SeTask { int read, slot; i64 cig_off; };   /* a gapped hit: slot -1 = the read's chosen hit, else its XA candidate multi[slot] */
+struct SeArgs {
+	int n_reads; i64 n_multi; int n_tasks;
+	int mode, max_top2; const char *rg; int l_rg;
+	TailCtg ctg; int n_holes; const i64 *amb_off; const int *amb_len;
+	const uint8_t *codes; const i64 *off;            /* the whole reads */
+	const bwag_se_read_t *reads; const bwag_se_hit_t *multi; const char *bc;
+	i64 *rows;                                        /* [n_reads + n_multi]: SA rows, resolved in place by K2 */
+	i64 *pos; uint8_t *strand, *mapped;               /* [n_reads]: bwa_sa2pos of the chosen hit (before refinement) */
+	i64 *mpos; uint8_t *mstrand, *mkeep;              /* [n_multi]: the candidates' positions; kept in XA */
+	const SeTask *tasks; const int *main_task, *multi_task;   /* the gapped hits; per read / candidate its task or -1 */
+	u32 *cig; int *ncig; int *tshift;                 /* per task: CIGAR at cig_off, its length (0: not run), the start's shift */
+	int *eh; uint8_t *rseq, *qseq, *z; int cap_q, cap_r; i64 cap_z;   /* per-warp scratch of the refinement */
+	int *next_task; int *past_end; u64 *n_run, *cells;
+	i64 *tlen; const i64 *tbeg; char *text; bwag_samrec_t *rec;   /* the records: bytes per read, their scan, the text */
+	int *nm;                                          /* [n_reads] NM of each mapped read, from pass 0 of S4 for pass 1 */
+};
+__global__ void k_se_rows(SeArgs a);
+__global__ void k_se_pos(SeArgs a);
+__global__ void k_se_refine(DevIndex ix, SeArgs a);
+__global__ void k_se_text(DevIndex ix, SeArgs a, int write);
+
 __global__ void k_chain_emit(ChainArgs a);
 __global__ void k_global_lane(DevIndex ix, GlbLaneArgs a);
 __global__ void k_localsw(DevIndex ix, SwArgs a);

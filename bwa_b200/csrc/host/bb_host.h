@@ -156,6 +156,45 @@ int bb_fastmap_main(int argc, char *argv[]);
 /* ---- `bwa-b200 aln` (bb_aln.c) ---- */
 int bb_aln_main(int argc, char *argv[]);
 
+/* ---- the reads of `aln` and `samse` (bb_seqio.c): bwa_read_seq, bwaseqio.c:151-221 ---- */
+#define BB_MODE_COMPREAD 0x02      /* the mode bits of gap_opt_t (bwtaln.h:94-103) */
+#define BB_MODE_CFY      0x08
+#define BB_MODE_BAM      0x20
+#define BB_MODE_IL13     0x200
+#define BB_MAX_BCLEN     63        /* BWA_MAX_BCLEN */
+#define BB_MIN_RDLEN     35        /* BWA_MIN_RDLEN: quality trimming stops here */
+typedef struct {
+	int n;
+	int64_t *off;              /* [n+1] first base of each read in codes[] */
+	uint8_t *codes;            /* keep == 0: the searched bases, 0..4; keep != 0: the whole read after the barcode, 0..5 (nst_nt4_table) */
+	int32_t *len;              /* [n] bases searched (after quality trimming) */
+	int max_len;               /* the most bases searched in one read */
+	int64_t *name, *qual, *bc; /* keep != 0: [n] offsets into text (NUL-terminated strings); qual / bc -1: none */
+	bb_str_t text;
+} bb_reads_t;
+/* gap_opt_t (bwtaln.h:105-115): the 64 bytes after "SAI\1" in a .sai file */
+typedef struct {
+	int32_t s_mm, s_gapo, s_gape;
+	int32_t mode;                 /* bits 24-31: barcode length */
+	int32_t indel_end_skip, max_del_occ, max_entries;
+	float fnr;
+	int32_t max_diff, max_gapo, max_gape;
+	int32_t max_seed_diff, seed_len;
+	int32_t n_threads;
+	int32_t max_top2;
+	int32_t trim_qual;
+} aln_opt_t;
+_Static_assert(sizeof(aln_opt_t) == 64, "gap_opt_t is 16 four-byte fields");
+_Static_assert(offsetof(aln_opt_t, mode) == 12 && offsetof(aln_opt_t, fnr) == 28 && offsetof(aln_opt_t, max_diff) == 32, "gap_opt_t layout");
+_Static_assert(offsetof(aln_opt_t, seed_len) == 48 && offsetof(aln_opt_t, n_threads) == 52 && offsetof(aln_opt_t, trim_qual) == 60, "gap_opt_t layout");
+/* up to n_max reads (one group of the reference); NULL at the end of the input.  A read with max_len or more bases to search is
+ * fatal (`who` names the command). */
+bb_reads_t *bb_read_group(bb_fq_t *fq, int mode, int trim_qual, int n_max, int keep, int max_len, const char *who);
+void bb_reads_free(bb_reads_t *g);
+
+/* ---- `bwa-b200 samse` (bb_samse.c) ---- */
+int bb_samse_main(int argc, char *argv[]);
+
 #ifdef __cplusplus
 }
 #endif

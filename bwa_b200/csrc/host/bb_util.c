@@ -8,6 +8,7 @@
 #include <sys/time.h>
 #include <sys/resource.h>
 #include <limits.h>
+#include <math.h>
 #include "bb_util.h"
 #include "bb_sort.h"
 
@@ -237,4 +238,21 @@ void *bb_mbox_get(bb_mbox_t *m)
 	pthread_cond_broadcast(&m->cv);
 	pthread_mutex_unlock(&m->mu);
 	return item;
+}
+
+/* bwa_cal_maxdiff (bwtaln.c:42-54): the smallest k with P(more than k errors in l bases) < thres for Poisson(l*err) errors, in the
+ * reference's double expression order and with its int factorial, which wraps past 12! (then k comes out of the wrapped values,
+ * as in the reference binary) */
+int bb_cal_maxdiff(int l, double err, double thres)
+{
+	const double elambda = exp(-l * err);
+	double sum = elambda, y = 1.0;
+	int k, x = 1;
+	for (k = 1; k < 1000; ++k) {
+		y *= l * err;
+		x = (int)((unsigned)x * (unsigned)k);
+		sum += elambda * y / x;
+		if (1.0 - sum < thres) return k;
+	}
+	return 2;
 }

@@ -57,6 +57,9 @@ void bb_mbox_init(bb_mbox_t *m);
 void bb_mbox_put(bb_mbox_t *m, void *item);
 void *bb_mbox_get(bb_mbox_t *m);
 
+/* bwa_cal_maxdiff (bwtaln.c:42-54): the most differences `bwa aln` allows in a read of l bases (-n as a fraction) */
+int bb_cal_maxdiff(int l, double err, double thres);
+
 typedef struct { uint64_t x, y; } bb_pair64_t;
 void bb_sort_u64(size_t n, uint64_t *a);         /* == ks_introsort_64 */
 void bb_sort_pair64(size_t n, bb_pair64_t *a);   /* == ks_introsort_128 (by x, then y) */

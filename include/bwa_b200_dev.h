@@ -260,6 +260,43 @@ typedef struct { const bwag_samrec_t *rec; const char *text; int64_t n_text, n_c
 int bwag_tail_sam(bwag_batch_t *b, const mem_opt_t *opt, const mem_pestat_t pes[4], const double *const pair_tab[4], const double *log_tab,
                   int64_t n_processed, const char *rg_id, bwag_sam_t *out);
 
+/* ---- single-end SAM of `bwa samse` (replaces bwa_cal_pac_pos, bwa_refine_gapped and bwa_print_sam1 with no mate,
+ * bwase.c:112-499) -------------------------------------------------------------------------------------------------------------
+ * The batch's codes are the whole reads after barcode removal (0..5, as nst_nt4_table gives them).  The caller has chosen each
+ * read's hit and its XA candidates (bwa_aln2seq_core, host, in read order: its random draws are serial) and its mapping quality.
+ * Per read, on the device: the positions of the chosen hit and of its candidates (bwa_sa2pos through the resident suffix array),
+ * the candidates that stay in XA, the banded global alignment of every gapped hit (ksw_global with the fix-ups of
+ * bwa_refine_gapped_core), MD and NM (bwa_cal_md1), the trimming correction (bwa_correct_trimmed) and the SAM record in the
+ * stage-4 layout (bwag_samrec_t; part B holds no trailing newline).  Needs bwag_ctx_set_contigs and bwag_ctx_set_ambs.
+ * BWAG_UNSUPPORTED from the CPU oracle of the tests. */
+#define BWAG_SE_COMPREAD 0x02   /* gap_opt_t mode bit: NM (else CM) and a complemented rseq */
+typedef struct {
+	uint64_t sa;                 /* the chosen suffix-array row */
+	int32_t len;                 /* bases searched (after quality trimming); the whole read is in the batch's codes */
+	int32_t clip_len;            /* XC:i: is printed when it is below the read's length */
+	int32_t ref_shift;           /* n_del - n_ins of the chosen hit */
+	uint8_t type, n_mm, n_gapo, n_gape;   /* 0 no match, 1 unique, 2 repeat; the chosen hit's differences */
+	uint32_t c1, c2;             /* X0 and X1: best and second-best hit counts (28 bits each, as bwa_seq_t keeps them) */
+	uint8_t mapq, l_bc, pad[2];
+	int32_t n_multi;             /* XA candidates: par->multi[multi_beg, multi_beg + n_multi), in bwa_aln2seq_core's order */
+	int64_t multi_beg;
+	int64_t bc_off;              /* the barcode: par->bc[bc_off, bc_off + l_bc) */
+} bwag_se_read_t;
+typedef struct { uint64_t sa; int32_t ref_shift; uint8_t gap, mm, pad[2]; } bwag_se_hit_t;   /* gap = n_gapo + n_gape (8 bits) */
+typedef struct {
+	int mode;                    /* BWAG_SE_COMPREAD */
+	int max_top2;                /* X1 is printed when X0 <= max_top2 */
+	const char *rg_id;           /* NULL or "": no RG tag */
+	const bwag_se_read_t *reads; /* [n_reads] */
+	const bwag_se_hit_t *multi; int64_t n_multi;
+	const char *bc; int64_t l_bc;
+} bwag_samse_par_t;
+/* the holes of the reference (bns->ambs): bns_cnt_ambi counts the N bases under an alignment for XN and XT */
+int bwag_ctx_set_ambs(bwag_ctx_t *ctx, int n_holes, const int64_t *offset, const int32_t *len);
+/* *past_end: -1, or the first read of the batch whose gapped alignment window runs past the end of the forward strand (the
+ * reference aborts on its assert there, bwase.c:180); the call then fails.  n_sa, n_glb: SA rows resolved, global alignments run. */
+int bwag_samse(bwag_batch_t *b, const bwag_samse_par_t *par, bwag_sam_t *out, int *past_end, int64_t *n_sa, int64_t *n_glb);
+
 /* ---- work / time counters for the roofline ---------------------------------------------------- */
 typedef struct {
 	uint64_t occ_touches;      /* 64-byte Occ blocks touched by bwt_extend (1 or 2 per call, bwt.c:194-197) */
