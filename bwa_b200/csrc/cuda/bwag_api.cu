@@ -54,6 +54,7 @@ struct Counters {
 	u64 t_dregs, t_tasks, t_max_z, t_text, t_complex;
 	int t_max_lq, t_max_rl;
 	int n_many;      /* reads with more chains than the lane kernel takes (K3) */
+	int n_big;       /* reads with more seeds than the on-chip form of K3 takes */
 	u32 n_swtasks;   /* local alignments the seed-level filter of long reads asks for (K3) */
 	u64 fm_total[3]; /* fastmap: lines, suffix-array rows and text bytes of the batch (totals of the scans) */
 	int aln_next;    /* aln: next read of the work list, reads listed for another run, why (1 arena, 2 pool), hits reserved in the pool, hits in all */
@@ -103,6 +104,7 @@ struct bwag_ctx {
 	/* scratch reused across batches */
 	DevBuf s_k1, s_k1f, s_n3, s_eh, s_rseq, s_qseq, s_z, s_wcig, s_wmd, s_pack, s_zl;
 	int grid_k1, grid_k1f, grid_k2, grid_k4, grid_k5;
+	int k3s_blocks;   /* resident blocks per SM of k_chain_sm (occupancy API) */
 #define N_SPARE 12
 	struct bwag_batch *spare[N_SPARE]; /* batch objects (stream, counters, scratch, device and pinned buffers) kept for later batches */
 	pthread_mutex_t mu;
@@ -139,6 +141,7 @@ struct bwag_batch {
 	DevBuf d_dregs, d_dreg_beg, d_dreg_n, d_task_beg, d_cflag, d_pe_is, d_rec, d_text, d_ptab;
 	DevBuf d_swtasks, d_swres, d_swpool, d_swscratch; HostBuf h_swres;   /* K6 */
 	DevBuf d_hsp, d_flt_nchn; HostBuf h_hsp;   /* seed-level filter of long reads (K3/K3b) */
+	DevBuf d_k3big;                            /* reads k_chain_sm leaves to k_chain */
 	DevBuf d_pre_n, d_pre_score, d_pre_cig;    /* K5L results for the warp kernel */
 	DevBuf d_sel;
 	HostBuf h_pe_is, h_cflag, h_rec, h_text, h_ptab;
@@ -232,6 +235,7 @@ static int pick_grid(bwag_ctx_t *c)
 #ifdef BWAG_CUSIM
 	c->n_sm = 2;
 	c->grid_k1 = c->grid_k1f = c->grid_k2 = c->grid_k4 = c->grid_k5 = 2;
+	c->k3s_blocks = 1;
 #else
 	cudaDeviceProp prop;
 	int nb;
@@ -239,6 +243,8 @@ static int pick_grid(bwag_ctx_t *c)
 	c->n_sm = prop.multiProcessorCount;
 	CK(cudaFuncSetAttribute(k_smem, cudaFuncAttributeMaxDynamicSharedMemorySize, K1_SMEM_MAX));
 	CK(cudaFuncSetAttribute(k_smem_fm, cudaFuncAttributeMaxDynamicSharedMemorySize, K1_SMEM_MAX));
+	CK(cudaFuncSetAttribute(k_chain_sm, cudaFuncAttributeMaxDynamicSharedMemorySize, K3S_SMEM));
+	CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&c->k3s_blocks, k_chain_sm, K3S_THREADS, K3S_SMEM));
 #ifndef K1_PACKED8
 	CK(cudaFuncSetAttribute(k_smem_c, cudaFuncAttributeMaxDynamicSharedMemorySize, K1_SMEM_MAX));
 #endif
@@ -575,6 +581,39 @@ extern "C" int bwag_is_emulator(void)
 extern "C" void bwag_stats_get(bwag_ctx_t *c, bwag_stats_t *s) { pthread_mutex_lock(&c->mu); *s = c->st; pthread_mutex_unlock(&c->mu); }
 extern "C" void bwag_stats_reset(bwag_ctx_t *c) { pthread_mutex_lock(&c->mu); memset(&c->st, 0, sizeof(c->st)); pthread_mutex_unlock(&c->mu); }
 
+/* K3 cycle histograms of a build with -DBWAG_K3_CLOCKS (tools/chain_bench.py): by seeds per read (0..64, then > 64) the reads and the
+ * clock64() cycles of their chaining loop, mem_chain_flt and chain_emit, then the reads by chains per read (0..32, then > 32) */
+#ifdef BWAG_K3_CLOCKS
+static pthread_mutex_t g_k3clk_mu = PTHREAD_MUTEX_INITIALIZER;
+static u64 g_k3clk[BWAG_K3CLK_WORDS];
+#endif
+extern "C" int bwag_k3_clocks(uint64_t *out, int reset)
+{
+#ifdef BWAG_K3_CLOCKS
+	pthread_mutex_lock(&g_k3clk_mu);
+	if (out) memcpy(out, g_k3clk, sizeof(g_k3clk));
+	if (reset) memset(g_k3clk, 0, sizeof(g_k3clk));
+	pthread_mutex_unlock(&g_k3clk_mu);
+	return 0;
+#else
+	(void)out; (void)reset;
+	return -1;
+#endif
+}
+#ifdef BWAG_K3_CLOCKS
+static void k3clk_add(const u32 *rec, int n)
+{
+	pthread_mutex_lock(&g_k3clk_mu);
+	for (int r = 0; r < n; ++r, rec += 5) {
+		const int t = rec[0] > 64 ? 65 : (int)rec[0], ch = rec[1] > 32 ? 33 : (int)rec[1];
+		u64 *h = g_k3clk + 4 * t;
+		h[0] += 1; h[1] += rec[2]; h[2] += rec[3]; h[3] += rec[4];
+		g_k3clk[4 * 66 + ch] += 1;
+	}
+	pthread_mutex_unlock(&g_k3clk_mu);
+}
+#endif
+
 extern "C" void *bwag_host_alloc(size_t bytes)
 {
 	void *p = 0;
@@ -606,6 +645,7 @@ extern "C" bwag_batch_t *bwag_batch_begin(bwag_ctx_t *c, int n, const uint8_t *c
 	b->lc.baseline = c->baseline;
 	if (c->baseline) { b->lc.ix.ktab = 0; b->lc.ix.ktab_k = 0; }
 	b->lc.grid_k1 = c->grid_k1; b->lc.grid_k1f = c->grid_k1f; b->lc.grid_k2 = c->grid_k2; b->lc.grid_k4 = c->grid_k4; b->lc.grid_k5 = c->grid_k5;
+	b->lc.k3s_blocks = c->k3s_blocks;
 	memset(&b->lc.st, 0, sizeof(b->lc.st));
 	b->max_len = 0; b->seeded = 0; b->tail_ready = 0; b->regs_on_device = 0;
 	b->ctx = c; b->n = n; b->h_off = (const i64 *)off; b->total_bases = off[n];
@@ -666,7 +706,7 @@ static void batch_free(bwag_batch_t *b)
 	free_dev(&b->d_tasks); free_dev(&b->d_res); free_dev(&b->d_cig); free_dev(&b->d_md);
 	free_host(&b->h_res); free_host(&b->h_cig); free_host(&b->h_md);
 	free_dev(&b->d_sel); free_dev(&b->d_swtasks); free_dev(&b->d_swres); free_dev(&b->d_swpool); free_dev(&b->d_swscratch); free_host(&b->h_swres);
-	free_dev(&b->d_hsp); free_dev(&b->d_flt_nchn); free_host(&b->h_hsp);
+	free_dev(&b->d_hsp); free_dev(&b->d_flt_nchn); free_host(&b->h_hsp); free_dev(&b->d_k3big);
 	free_dev(&b->d_pre_n); free_dev(&b->d_pre_score); free_dev(&b->d_pre_cig);
 	free_dev(&b->d_dregs); free_dev(&b->d_dreg_beg); free_dev(&b->d_dreg_n); free_dev(&b->d_task_beg); free_dev(&b->d_cflag); free_dev(&b->d_pe_is); free_dev(&b->d_rec); free_dev(&b->d_text); free_dev(&b->d_ptab);
 	free_host(&b->h_pe_is); free_host(&b->h_cflag); free_host(&b->h_rec); free_host(&b->h_text); free_host(&b->h_ptab);
@@ -1505,7 +1545,7 @@ extern "C" int bwag_chain_extend(bwag_batch_t *b, const bwag_chain_par_t *cp, co
 	    buf_reserve(&b->d_chains, sizeof(bwag_xchain_t) * (size_t)(ns + 1)) || buf_reserve(&b->d_seeds, sizeof(bwag_xseed_t) * (size_t)(ns + 1)) ||
 	    buf_reserve(&b->d_regs, sizeof(bwag_xreg_t) * (size_t)(ns + 1)) || buf_reserve(&b->d_chain_rid, 4 * (size_t)(ns + 1)) || buf_reserve(&b->d_chain_frac, 4 * (size_t)(ns + 1)) ||
 	    buf_reserve(&b->d_chain_beg, 8 * (size_t)(n + 1)) || buf_reserve(&b->d_chain_cnt, 4 * (size_t)(n + 1)) || buf_reserve(&b->d_reg_base, 8 * (size_t)(n + 1)) ||
-	    buf_reserve(&b->d_nregs, 4 * (size_t)(n + 1)) || buf_reserve(&b->d_creg_beg, 8 * (size_t)(n + 1))) return 1;
+	    buf_reserve(&b->d_nregs, 4 * (size_t)(n + 1)) || buf_reserve(&b->d_creg_beg, 8 * (size_t)(n + 1)) || buf_reserve(&b->d_k3big, 4 * (size_t)(n + 1))) return 1;
 	if (reset_counters(c)) return 1;
 	H2D(c, b->d_ctg.p, b->h_tmp.p, 13 * (size_t)ctg->n_seqs);
 	ChainArgs k;
@@ -1541,12 +1581,41 @@ extern "C" int bwag_chain_extend(bwag_batch_t *b, const bwag_chain_par_t *cp, co
 			k.sw_tasks = (bwag_swtask_t *)b->d_swtasks.p; k.n_swtasks = &c->d_cnt->n_swtasks;
 		} else if (any) return BWAG_DECLINED;   /* switched off: the caller chains these reads on the host */
 	}
+#ifdef BWAG_K3_CLOCKS
+	CK(cudaMalloc((void **)&k.k3clk, 20 * (size_t)(n + 1)));
+#endif
+	/* Without the long-read filter, k_chain_sm chains the reads with few seeds in shared memory and lists the others, which
+	 * k_chain then takes with their workspace in HBM (grid-stride over the list, whose length only the device knows).  With the
+	 * filter every read takes k_chain: K3b reads the HBM workspace back. */
+	const int on_chip = !k.hsp_tab;
+	int k3_grid = (n + K3_THREADS - 1) / K3_THREADS;
+	if (on_chip) {
+		k.big = (int *)b->d_k3big.p; k.n_big = &c->d_cnt->n_big;
+		if (k3_grid > c->n_sm * 16) k3_grid = c->n_sm * 16;
+	}
 	CK(cudaEventRecord(c->ev0, c->stream));
-	BWAG_LAUNCH(k_chain, (n + K3_THREADS - 1) / K3_THREADS, K3_THREADS, 0, c->stream, k);
+	if (on_chip) {
+		BWAG_LAUNCH(k_chain_sm, (n + K3S_THREADS - 1) / K3S_THREADS, K3S_THREADS, K3S_SMEM, c->stream, k);
+		CK(cudaGetLastError());
+	}
+	BWAG_LAUNCH(k_chain, k3_grid > 0 ? k3_grid : 1, K3_THREADS, 0, c->stream, k);
 	CK(cudaGetLastError());
 	CK(cudaEventRecord(c->ev1, c->stream));
 	if (fetch_counters(c)) return 1;
-	c->st.ms_chain += elapsed_at(c, "chain", __LINE__); ++c->st.n_launch;
+	c->st.ms_chain += elapsed_at(c, "chain", __LINE__); c->st.n_launch += 1 + on_chip;
+	if (getenv("BWA_B200_PROFILE"))
+		fprintf(stderr, "[prof] chain: %d reads on chip, %d in HBM, CAP %d seeds, %d blocks of %d threads per SM on chip\n",
+		        on_chip ? n - c->h_cnt->n_big : 0, on_chip ? c->h_cnt->n_big : n, K3S_CAP, c->k3s_blocks, K3S_THREADS);
+#ifdef BWAG_K3_CLOCKS
+	{
+		u32 *h = (u32 *)malloc(20 * (size_t)(n + 1));
+		CK(cudaMemcpy(h, k.k3clk, 20 * (size_t)n, cudaMemcpyDeviceToHost));
+		CK(cudaFree(k.k3clk));
+		k.k3clk = 0;
+		k3clk_add(h, n);
+		free(h);
+	}
+#endif
 	if (k.hsp_tab) {
 		const int n_sw = (int)c->h_cnt->n_swtasks;
 		if (n_sw > 0) {

@@ -145,4 +145,32 @@ struct SmemAcc {
 #define BWAG_KEEP(x) asm volatile("" : "+r"(x))   /* the value stays in its register: no re-derivation inside the loops */
 #endif
 
+/* ks_introsort (ksort.h:176-226) for n <= 17: the depth budget never runs out and neither side of the first partition
+ * is deferred or iterated on (both have <= 16 gaps), so the procedure is ONE median-of-three partition followed by the
+ * closing insertion sort -- move for move what the reference executes, hence the same order among equal keys.
+ * A is anything indexable that yields an lvalue: a pointer, or a strided view of a shared-memory array (K3). */
+template <class A, class LT>
+__device__ void t_isort17(A a, int n, LT lt)
+{
+	if (n < 2) return;
+	if (n == 2) { if (lt(a[1], a[0])) { auto x = a[0]; a[0] = a[1]; a[1] = x; } return; }
+	{
+		int i = 0, j = n - 1, k = ((n - 1) >> 1) + 1;
+		const int hi = n - 1;
+		if (lt(a[k], a[i])) { if (lt(a[k], a[j])) k = j; }
+		else k = lt(a[j], a[i]) ? i : j;
+		const auto piv = a[k];
+		if (k != hi) { auto x = a[k]; a[k] = a[hi]; a[hi] = x; }
+		for (;;) {
+			do ++i; while (lt(a[i], piv));
+			do --j; while (i <= j && lt(piv, a[j]));
+			if (j <= i) break;
+			{ auto x = a[i]; a[i] = a[j]; a[j] = x; }
+		}
+		{ auto x = a[i]; a[i] = a[hi]; a[hi] = x; }
+	}
+	for (int p = 1; p < n; ++p)
+		for (int q = p; q > 0 && lt(a[q], a[q - 1]); --q) { auto x = a[q]; a[q] = a[q - 1]; a[q - 1] = x; }
+}
+
 #endif

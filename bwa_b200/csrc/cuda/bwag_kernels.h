@@ -17,6 +17,13 @@
 #define K1B_THREADS 128
 #define K2_THREADS 128
 #define K3_THREADS 128
+/* K3 on chip (k_chain_sm): reads with at most K3S_CAP seeds keep their chaining workspace in K3S_SMEM bytes of shared memory per
+ * block (62 bytes per seed, 21 per B-tree node, 4 of traversal stack, per lane; bwag_chain.cu) */
+#ifndef K3S_CAP
+#define K3S_CAP 16
+#endif
+#define K3S_THREADS 64
+#define K3S_SMEM (K3S_THREADS * (62 * K3S_CAP + 21 * (1 + (K3S_CAP - 1) / 4) + 4))
 #define K4_THREADS 128
 #define K5_THREADS 128
 #define K4L_THREADS 128   /* lane-per-read extension kernel (bwag_extend_lane.cu) */
@@ -67,6 +74,8 @@ struct ChainArgs {
 	/* seed-level filter of long reads (mem_flt_chained_seeds): threshold by read length (-1: inactive; NULL: no read of the chunk is
 	 * long enough), the local alignments k_chain asks for, their results for k_chain_emit, per read the number of chains parked */
 	const int *hsp_tab; bwag_swtask_t *sw_tasks; u32 *n_swtasks; const bwag_swres_t *sw_res; int *flt_nchn;
+	int *big; int *n_big;                                              /* reads k_chain_sm leaves to k_chain (too many seeds), their count */
+	u32 *k3clk;   /* builds with -DBWAG_K3_CLOCKS only: per read seeds, chains, cycles of chaining, mem_chain_flt, chain_emit */
 };
 
 struct RegCompactArgs {
@@ -267,6 +276,7 @@ __global__ void k_sa(DevIndex ix, SaArgs a);
 __global__ void k_sa_densify(DevIndex ix, u64 *out, int out_shift, u64 n_out);
 __global__ void k_index_verify(DevIndex ix, u64 first, u64 stride, u64 n_check, u64 *out);
 __global__ void k_chain(ChainArgs a);
+__global__ void k_chain_sm(ChainArgs a);
 __global__ void k_regs_compact(RegCompactArgs a);
 __global__ void k_regs_compact_sel(RegCompactArgs a, const int *sel, int n_sel, int *out_n);
 __global__ void k_extend(DevIndex ix, ExtArgs a);

@@ -49,32 +49,6 @@ __device__ __forceinline__ int t_infer_dir(i64 l_pac, i64 b1, i64 b2, i64 *dist)
 	return (r1 == r2 ? 0 : 1) ^ (p2 > b1 ? 0 : 3);
 }
 
-/* ks_introsort (ksort.h:176-226) for n <= 17: the depth budget never runs out and neither side of the first partition
- * is deferred or iterated on (both have <= 16 gaps), so the procedure is ONE median-of-three partition followed by the
- * closing insertion sort -- move for move what the reference executes, hence the same order among equal keys. */
-template <class T, class LT>
-__device__ void t_isort17(T *a, int n, LT lt)
-{
-	if (n < 2) return;
-	if (n == 2) { if (lt(a[1], a[0])) { T x = a[0]; a[0] = a[1]; a[1] = x; } return; }
-	{
-		int i = 0, j = n - 1, k = ((n - 1) >> 1) + 1;
-		const int hi = n - 1;
-		if (lt(a[k], a[i])) { if (lt(a[k], a[j])) k = j; }
-		else k = lt(a[j], a[i]) ? i : j;
-		const T piv = a[k];
-		if (k != hi) { T x = a[k]; a[k] = a[hi]; a[hi] = x; }
-		for (;;) {
-			do ++i; while (lt(a[i], piv));
-			do --j; while (i <= j && lt(piv, a[j]));
-			if (j <= i) break;
-			{ T x = a[i]; a[i] = a[j]; a[j] = x; }
-		}
-		{ T x = a[i]; a[i] = a[hi]; a[hi] = x; }
-	}
-	for (int p = 1; p < n; ++p)
-		for (int q = p; q > 0 && lt(a[q], a[q - 1]); --q) { T x = a[q]; a[q] = a[q - 1]; a[q - 1] = x; }
-}
 struct LtEnd { __device__ bool operator()(const mem_alnreg_t &a, const mem_alnreg_t &b) const { return a.re < b.re; } };
 struct LtScorePos { __device__ bool operator()(const mem_alnreg_t &a, const mem_alnreg_t &b) const { return a.score > b.score || (a.score == b.score && (a.rb < b.rb || (a.rb == b.rb && a.qb < b.qb))); } };
 struct LtScoreHash { __device__ bool operator()(const mem_alnreg_t &a, const mem_alnreg_t &b) const { return a.score > b.score || (a.score == b.score && (a.is_alt < b.is_alt || (a.is_alt == b.is_alt && a.hash < b.hash))); } };

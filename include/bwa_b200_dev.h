@@ -316,6 +316,11 @@ typedef struct {
 } bwag_stats_t;
 void bwag_stats_get(bwag_ctx_t *ctx, bwag_stats_t *s);
 void bwag_stats_reset(bwag_ctx_t *ctx);
+/* builds with -DBWAG_K3_CLOCKS only (else returns -1): copies the chaining kernel's cycle histograms (BWAG_K3CLK_WORDS words) to out,
+ * then clears them if reset.  Words 4t..4t+3, t = seeds per read (0..64, 65: more): reads, cycles of the chaining loop, of
+ * mem_chain_flt, of chain_emit; words 264+c, c = chains per read (0..32, 33: more): reads. */
+#define BWAG_K3CLK_WORDS (4 * 66 + 34)
+int bwag_k3_clocks(uint64_t *out, int reset);
 
 #ifdef __cplusplus
 }
