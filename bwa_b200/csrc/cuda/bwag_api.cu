@@ -154,6 +154,9 @@ struct bwag_batch {
 	/* samse (bwag_samse.cu) */
 	DevBuf d_se_reads, d_se_multi, d_se_bc, d_se_rows, d_se_pos, d_se_mpos, d_se_flags, d_se_tasks, d_se_mtask, d_se_cig, d_se_ncig, d_se_scratch, d_se_tlen, d_se_tbeg, d_se_rec, d_se_text, d_se_nm;
 	HostBuf h_se_tasks, h_se_mtask, h_se_rec, h_se_text;
+	/* sampe (bwag_sampe.cu; the rest of its buffers are samse's) */
+	DevBuf d_pe_rlen, d_pe_reads, d_pe_gtasks, d_pe_gres, d_pe_gcig, d_pe_pool;
+	HostBuf h_pe_pos, h_pe_gres, h_pe_gcig;
 	int tail_ready;             /* bwag_tail_regs ran on this batch */
 	int regs_on_device;          /* bwag_chain_extend left the regions in HBM */
 };
@@ -717,6 +720,8 @@ static void batch_free(bwag_batch_t *b)
 	free_dev(&b->d_se_reads); free_dev(&b->d_se_multi); free_dev(&b->d_se_bc); free_dev(&b->d_se_rows); free_dev(&b->d_se_pos); free_dev(&b->d_se_mpos); free_dev(&b->d_se_flags);
 	free_dev(&b->d_se_tasks); free_dev(&b->d_se_mtask); free_dev(&b->d_se_cig); free_dev(&b->d_se_ncig); free_dev(&b->d_se_scratch); free_dev(&b->d_se_tlen); free_dev(&b->d_se_tbeg);
 	free_dev(&b->d_se_rec); free_dev(&b->d_se_text); free_dev(&b->d_se_nm); free_host(&b->h_se_tasks); free_host(&b->h_se_mtask); free_host(&b->h_se_rec); free_host(&b->h_se_text);
+	free_dev(&b->d_pe_rlen); free_dev(&b->d_pe_reads); free_dev(&b->d_pe_gtasks); free_dev(&b->d_pe_gres); free_dev(&b->d_pe_gcig); free_dev(&b->d_pe_pool);
+	free_host(&b->h_pe_pos); free_host(&b->h_pe_gres); free_host(&b->h_pe_gcig);
 	free(b);
 }
 
@@ -1316,6 +1321,238 @@ extern "C" int bwag_samse(bwag_batch_t *b, const bwag_samse_par_t *par, bwag_sam
 	CK(cudaEventRecord(c->ev0, c->stream));
 	if (n_text) D2H(c, b->h_se_text.p, b->d_se_text.p, (size_t)n_text);
 	if (n) D2H(c, b->h_se_rec.p, b->d_se_rec.p, sizeof(bwag_samrec_t) * (size_t)n);
+	CK(cudaEventRecord(c->ev1, c->stream));
+	CK(stream_wait(c));
+	c->st.ms_d2h += elapsed_at(c, "d2h", __LINE__);
+	out->rec = (const bwag_samrec_t *)b->h_se_rec.p; out->text = (const char *)b->h_se_text.p; out->n_text = n_text;
+	return 0;
+}
+
+/* ------------------------------------------------------------------------------------------------ sampe */
+
+/* P1/P2: K2 resolves the rows in place, k_pe_pos applies bwa_sa2pos twice per row */
+extern "C" int bwag_pe_sa2pos(bwag_batch_t *b, int64_t n_rows, const uint64_t *rows, const int32_t *ref_len, int64_t *pos, uint8_t *strand)
+{
+	bwag_ctx_t *c = &b->lc;
+	CK(cudaSetDevice(c->device));
+	if (n_rows <= 0) return 0;
+	const size_t n = (size_t)n_rows;
+	if (buf_reserve(&b->d_se_rows, 8 * n) || buf_reserve(&b->d_pe_rlen, 8 * n) || buf_reserve(&b->d_se_pos, 16 * n) || buf_reserve(&b->d_se_flags, 2 * n + 16) ||
+	    hbuf_reserve(&b->h_pe_pos, 18 * n + 16)) return 1;
+	PePosArgs a;
+	a.n = n_rows; a.l_pac = (i64)c->ix.l_pac; a.rows = (const i64 *)b->d_se_rows.p; a.ref_len = (const int *)b->d_pe_rlen.p;
+	a.pos = (i64 *)b->d_se_pos.p; a.strand = (uint8_t *)b->d_se_flags.p;
+	if (reset_counters(c)) return 1;
+	H2D(c, b->d_se_rows.p, rows, 8 * n);
+	H2D(c, b->d_pe_rlen.p, ref_len, 8 * n);
+	SaArgs sa;
+	sa.rbeg = (i64 *)b->d_se_rows.p; sa.n = n_rows; sa.next = &c->d_cnt->next_seed; sa.sa_touches = &c->d_cnt->sa_touches;
+	int grid = c->grid_k2;
+	const i64 need = (n_rows + K2_THREADS - 1) / K2_THREADS;
+	if (grid > need) grid = (int)need;
+	CK(cudaEventRecord(c->ev0, c->stream));
+	BWAG_LAUNCH(k_sa, grid, K2_THREADS, 0, c->stream, c->ix, sa);
+	CK(cudaEventRecord(c->ev1, c->stream));
+	BWAG_LAUNCH(k_pe_pos, fm_grid(c, n_rows), 128, 0, c->stream, a);
+	CK(cudaGetLastError());
+	c->st.n_launch += 2;
+	char *h = (char *)b->h_pe_pos.p;
+	D2H(c, h, b->d_se_pos.p, 16 * n);
+	D2H(c, h + 16 * n, b->d_se_flags.p, 2 * n);
+	CK(stream_wait(c));
+	c->st.ms_sa += elapsed_at(c, "sa", __LINE__);
+	memcpy(pos, h, 16 * n); memcpy(strand, h + 16 * n, 2 * n);
+	return 0;
+}
+
+/* P5: the global alignments of the accepted local ones, one warp each, as many warps as the scratch budget allows */
+extern "C" int bwag_pe_global(bwag_batch_t *b, int n_tasks, const bwag_pe_gtask_t *tasks, const uint8_t *pool, size_t pool_bytes, const bwag_pe_gres_t **res, const uint32_t **cig)
+{
+	bwag_ctx_t *c = &b->lc;
+	CK(cudaSetDevice(c->device));
+	*res = 0; *cig = 0;
+	if (n_tasks <= 0) return 0;
+	int cap_q = 1, cap_r = 1;
+	i64 cap_z = 1, n_cig = 0;
+	if (hbuf_reserve(&b->h_pe_gres, sizeof(bwag_pe_gres_t) * (size_t)n_tasks)) return 1;
+	bwag_pe_gres_t *hr = (bwag_pe_gres_t *)b->h_pe_gres.p;
+	for (int t = 0; t < n_tasks; ++t) {
+		const bwag_pe_gtask_t &tk = tasks[t];
+		if (tk.qlen < 1 || tk.tlen < 1 || tk.q_beg < 0 || tk.q_beg + tk.qlen > (i64)pool_bytes || tk.t_beg < 0 || tk.t_beg + tk.tlen > (i64)c->ix.l_pac)
+			return set_err("mate-rescue alignment %d: query [%lld, +%d) or target [%lld, +%d) out of range", t, (long long)tk.q_beg, tk.qlen, (long long)tk.t_beg, tk.tlen);
+		const int n_col = tk.qlen < 101 ? tk.qlen : 101;
+		hr[t].score = 0; hr[t].n_cigar = 0; hr[t].cig_off = n_cig;
+		n_cig += (i64)tk.qlen + tk.tlen + 2;
+		if (tk.qlen > cap_q) cap_q = tk.qlen;
+		if (tk.tlen > cap_r) cap_r = tk.tlen;
+		if ((i64)n_col * tk.tlen > cap_z) cap_z = (i64)n_col * tk.tlen;
+	}
+	if (buf_reserve(&b->d_pe_gtasks, sizeof(bwag_pe_gtask_t) * (size_t)n_tasks) || buf_reserve(&b->d_pe_gres, sizeof(bwag_pe_gres_t) * (size_t)n_tasks) ||
+	    buf_reserve(&b->d_pe_gcig, 4 * (size_t)n_cig) || buf_reserve(&b->d_pe_pool, pool_bytes + 16) || hbuf_reserve(&b->h_pe_gcig, 4 * (size_t)n_cig)) return 1;
+	const i64 per_warp = (8 * ((i64)cap_q + 2) + cap_r + cap_z + 15) & ~(i64)15;
+	i64 warps = (i64)c->n_sm * SE_WARPS_PER_SM;
+	if (warps > n_tasks) warps = n_tasks;
+	if (warps > SE_BUDGET / per_warp) warps = SE_BUDGET / per_warp;
+	if (warps < 1) warps = 1;
+	warps = (warps + 3) & ~(i64)3;   /* whole blocks of SE_THREADS */
+	if (buf_reserve(&b->d_se_scratch, (size_t)(warps * per_warp))) return 1;
+	PeGlbArgs a;
+	unsigned char *sc = (unsigned char *)b->d_se_scratch.p;
+	a.n_tasks = n_tasks; a.tasks = (const bwag_pe_gtask_t *)b->d_pe_gtasks.p; a.res = (bwag_pe_gres_t *)b->d_pe_gres.p; a.cig = (u32 *)b->d_pe_gcig.p;
+	a.pool = (const uint8_t *)b->d_pe_pool.p;
+	a.eh = (int *)sc; sc += warps * 8 * ((i64)cap_q + 2);
+	a.rseq = sc; sc += warps * (i64)cap_r;
+	a.z = sc;
+	a.cap_q = cap_q; a.cap_r = cap_r; a.cap_z = cap_z;
+	a.next_task = &c->d_cnt->se_next; a.cells = &c->d_cnt->se_cells;
+	if (reset_counters(c)) return 1;
+	H2D(c, b->d_pe_gtasks.p, tasks, sizeof(bwag_pe_gtask_t) * (size_t)n_tasks);
+	H2D(c, b->d_pe_gres.p, hr, sizeof(bwag_pe_gres_t) * (size_t)n_tasks);
+	H2D(c, b->d_pe_pool.p, pool, pool_bytes);
+	BWAG_LAUNCH(k_pe_global, (int)(warps * 32 / SE_THREADS), SE_THREADS, 0, c->stream, c->ix, a);
+	CK(cudaGetLastError());
+	++c->st.n_launch;
+	D2H(c, b->h_pe_gres.p, b->d_pe_gres.p, sizeof(bwag_pe_gres_t) * (size_t)n_tasks);
+	D2H(c, b->h_pe_gcig.p, b->d_pe_gcig.p, 4 * (size_t)n_cig);
+	if (fetch_counters(c)) return 1;
+	c->st.glb_cells += c->h_cnt->se_cells;
+	*res = (const bwag_pe_gres_t *)b->h_pe_gres.p; *cig = (const uint32_t *)b->h_pe_gcig.p;
+	return 0;
+}
+
+/* P6 (samse's S3 on the caller's positions) and P7, around a scan */
+extern "C" int bwag_sampe(bwag_batch_t *b, const bwag_sampe_par_t *par, bwag_sam_t *out, int *past_end, int64_t *n_glb)
+{
+	bwag_ctx_t *c = &b->lc, *pc = b->ctx;
+	CK(cudaSetDevice(c->device));
+	memset(out, 0, sizeof(*out));
+	*past_end = -1; *n_glb = 0;
+	if (!pc->have_ctg || !pc->have_ambs) return set_err("bwag_sampe needs the contig table and the holes (bwag_ctx_set_contigs, bwag_ctx_set_ambs)");
+	const int n = b->n;
+	if (n & 1) return set_err("bwag_sampe: a batch of %d reads is not a batch of pairs", n);
+	const i64 nm = par->n_multi, n_rows = (i64)n + nm;
+	if (hbuf_reserve(&b->h_se_tasks, sizeof(SeTask) * ((size_t)n_rows + 1)) || hbuf_reserve(&b->h_se_mtask, 4 * ((size_t)n_rows + 1))) return 1;
+	SeTask *tasks = (SeTask *)b->h_se_tasks.p;
+	int *mtask = (int *)b->h_se_mtask.p;
+	int n_tasks = 0, cap_q = 1, cap_r = 1;
+	i64 n_cig = 0, cap_z = 1;
+	int n_tasks1 = 0;   /* the tasks of end 1 come first: each end's rseq is complemented as its own .sai says */
+	for (int e = 0; e < 2; ++e) for (int r = e; r < n; r += 2) {
+		if (e == 1 && r == 1) n_tasks1 = n_tasks;
+		const bwag_se_read_t &p = par->reads[r];
+		if (p.len < 1 || p.len > (int)(b->h_off[r + 1] - b->h_off[r])) return set_err("read %d of the batch: %d bases searched of %lld", r, p.len, (long long)(b->h_off[r + 1] - b->h_off[r]));
+		for (int k = -1; k < p.n_multi; ++k) {
+			const i64 slot = k < 0 ? -1 : p.multi_beg + k;
+			int &mt = k < 0 ? mtask[r] : mtask[n + slot];
+			mt = -1;
+			if (k < 0 ? !((p.type == 1 || p.type == 2) && p.n_gapo) : !par->multi[slot].gap) continue;
+			const int rlen = p.len + (k < 0 ? p.ref_shift : par->multi[slot].ref_shift);
+			if (rlen < 0) return set_err("read %d of the batch: a gapped hit with %d reference bases", r, rlen);
+			int w = (int)(abs(rlen - p.len) * 1.5);
+			w = w > 50 ? w : 50;
+			const i64 n_col = p.len < 2 * w + 1 ? p.len : 2 * w + 1;
+			mt = n_tasks;
+			tasks[n_tasks].read = r; tasks[n_tasks].slot = (int)slot; tasks[n_tasks].cig_off = n_cig;
+			++n_tasks;
+			n_cig += (i64)p.len + rlen + 2;
+			if (p.len > cap_q) cap_q = p.len;
+			if (rlen > cap_r) cap_r = rlen;
+			if (n_col * rlen > cap_z) cap_z = n_col * rlen;
+		}
+	}
+	const i64 cig_base = n_cig;   /* the mate-rescued CIGARs follow the refinement's */
+	n_cig += par->n_cig;
+	const size_t l_rg = par->rg_id ? strlen(par->rg_id) : 0;
+	if (buf_reserve(&b->d_se_reads, sizeof(bwag_se_read_t) * ((size_t)n + 1)) || buf_reserve(&b->d_se_multi, sizeof(bwag_se_hit_t) * ((size_t)nm + 1)) ||
+	    buf_reserve(&b->d_pe_reads, sizeof(bwag_pe_read_t) * ((size_t)n + 1)) ||
+	    buf_reserve(&b->d_se_bc, (size_t)par->l_bc + l_rg + 16) ||
+	    buf_reserve(&b->d_se_pos, 8 * ((size_t)n + 1)) || buf_reserve(&b->d_se_mpos, 8 * ((size_t)nm + 1)) || buf_reserve(&b->d_se_flags, 2 * (size_t)n_rows + 16) ||
+	    buf_reserve(&b->d_se_tasks, sizeof(SeTask) * ((size_t)n_tasks + 1)) || buf_reserve(&b->d_se_mtask, 4 * ((size_t)n_rows + 1)) ||
+	    buf_reserve(&b->d_se_cig, 4 * ((size_t)n_cig + 1)) || buf_reserve(&b->d_se_ncig, 8 * ((size_t)n_tasks + 1)) ||
+	    buf_reserve(&b->d_se_tlen, 8 * ((size_t)n + 1)) || buf_reserve(&b->d_se_tbeg, 8 * ((size_t)n + 1)) || buf_reserve(&b->d_se_nm, 4 * ((size_t)n + 1)) || buf_reserve(&b->d_se_rec, sizeof(bwag_samrec_t) * ((size_t)n + 1)) ||
+	    hbuf_reserve(&b->h_se_rec, sizeof(bwag_samrec_t) * ((size_t)n + 1)) || hbuf_reserve(&b->h_pe_gres, sizeof(bwag_pe_read_t) * ((size_t)n + 1))) return 1;
+	bwag_pe_read_t *pe = (bwag_pe_read_t *)b->h_pe_gres.p;   /* the caller's, with the rescued CIGARs moved behind the refinement's */
+	for (int r = 0; r < n; ++r) { pe[r] = par->pe[r]; if (par->reads[r].type == 3) pe[r].cig_off += cig_base; }
+	SeArgs a;
+	memset(&a, 0, sizeof(a));
+	a.n_reads = n; a.n_multi = nm; a.n_tasks = n_tasks; a.mode = par->mode; a.max_top2 = par->max_top2;
+	a.ctg = pc->tctg; a.n_holes = pc->n_holes; a.amb_off = (const i64 *)pc->d_ambs; a.amb_len = (const int *)((const char *)pc->d_ambs + 8 * (size_t)pc->n_holes);
+	a.codes = (const uint8_t *)b->d_codes.p; a.off = (const i64 *)b->d_off.p;
+	a.reads = (const bwag_se_read_t *)b->d_se_reads.p; a.multi = (const bwag_se_hit_t *)b->d_se_multi.p;
+	a.bc = (const char *)b->d_se_bc.p; a.rg = (const char *)b->d_se_bc.p + par->l_bc; a.l_rg = (int)l_rg;
+	a.pos = (i64 *)b->d_se_pos.p; a.mpos = (i64 *)b->d_se_mpos.p;
+	a.strand = (uint8_t *)b->d_se_flags.p; a.mapped = a.strand + n; a.mstrand = a.mapped + n; a.mkeep = a.mstrand + nm;
+	a.tasks = (const SeTask *)b->d_se_tasks.p; a.main_task = (const int *)b->d_se_mtask.p; a.multi_task = a.main_task + n;
+	a.cig = (u32 *)b->d_se_cig.p; a.ncig = (int *)b->d_se_ncig.p; a.tshift = a.ncig + n_tasks;
+	a.next_task = &c->d_cnt->se_next; a.past_end = &c->d_cnt->se_past; a.n_run = &c->d_cnt->se_run; a.cells = &c->d_cnt->se_cells;
+	a.tlen = (i64 *)b->d_se_tlen.p; a.tbeg = (const i64 *)b->d_se_tbeg.p; a.rec = (bwag_samrec_t *)b->d_se_rec.p; a.nm = (int *)b->d_se_nm.p;
+	if (reset_counters(c)) return 1;
+	{   /* mapped[] (type 1 or 2: refined when gapped) and mkeep[] (every candidate given), in pinned memory for the copy */
+		if (hbuf_reserve(&b->h_pe_pos, (size_t)n + (size_t)nm + 16)) return 1;
+		uint8_t *f = (uint8_t *)b->h_pe_pos.p;
+		for (int r = 0; r < n; ++r) f[r] = par->reads[r].type == 1 || par->reads[r].type == 2;
+		memset(f + n, 1, (size_t)nm);
+		H2D(c, a.mapped, f, (size_t)n);
+		if (nm) H2D(c, a.mkeep, f + n, (size_t)nm);
+	}
+	H2D(c, b->d_se_reads.p, par->reads, sizeof(bwag_se_read_t) * (size_t)n);
+	H2D(c, b->d_pe_reads.p, pe, sizeof(bwag_pe_read_t) * (size_t)n);
+	H2D(c, a.pos, par->pos, 8 * (size_t)n);
+	H2D(c, a.strand, par->strand, (size_t)n);
+	if (nm) { H2D(c, b->d_se_multi.p, par->multi, sizeof(bwag_se_hit_t) * (size_t)nm); H2D(c, a.mpos, par->mpos, 8 * (size_t)nm); H2D(c, a.mstrand, par->mstrand, (size_t)nm); }
+	if (par->n_cig) H2D(c, a.cig + cig_base, par->cig, 4 * (size_t)par->n_cig);
+	if (par->l_bc) H2D(c, b->d_se_bc.p, par->bc, (size_t)par->l_bc);
+	if (l_rg) H2D(c, (char *)b->d_se_bc.p + par->l_bc, par->rg_id, l_rg);
+	if (n_tasks) H2D(c, b->d_se_tasks.p, tasks, sizeof(SeTask) * (size_t)n_tasks);
+	H2D(c, b->d_se_mtask.p, mtask, 4 * (size_t)n_rows);
+	if (n_tasks) {
+		const i64 per_warp = (8 * ((i64)cap_q + 2) + cap_r + cap_q + cap_z + 15) & ~(i64)15;
+		i64 warps = (i64)c->n_sm * SE_WARPS_PER_SM;
+		if (warps > n_tasks) warps = n_tasks;
+		if (warps > SE_BUDGET / per_warp) warps = SE_BUDGET / per_warp;
+		if (warps < 1) warps = 1;
+		warps = (warps + 3) & ~(i64)3;
+		if (buf_reserve(&b->d_se_scratch, (size_t)(warps * per_warp))) return 1;
+		unsigned char *sc = (unsigned char *)b->d_se_scratch.p;
+		a.eh = (int *)sc; sc += warps * 8 * ((i64)cap_q + 2);
+		a.rseq = sc; sc += warps * (i64)cap_r;
+		a.qseq = sc; sc += warps * (i64)cap_q;
+		a.z = sc;
+		a.cap_q = cap_q; a.cap_r = cap_r; a.cap_z = cap_z;
+		CK(cudaMemsetAsync(b->d_se_ncig.p, 0, 8 * (size_t)n_tasks, c->stream));
+		for (int e = 0; e < 2; ++e) {   /* S3 once per end, with that end's COMPREAD bit */
+			const int t0 = e ? n_tasks1 : 0, nt = e ? n_tasks - n_tasks1 : n_tasks1;
+			if (!nt) continue;
+			SeArgs ae = a;
+			ae.tasks = a.tasks + t0; ae.ncig = a.ncig + t0; ae.tshift = a.tshift + t0; ae.n_tasks = nt;
+			ae.mode = par->comp[e] ? BWAG_SE_COMPREAD : 0;
+			CK(cudaMemsetAsync(&c->d_cnt->se_next, 0, sizeof(int), c->stream));
+			BWAG_LAUNCH(k_se_refine, (int)(warps * 32 / SE_THREADS), SE_THREADS, 0, c->stream, c->ix, ae);
+			CK(cudaGetLastError());
+			++c->st.n_launch;
+		}
+	}
+	const bwag_pe_read_t *d_pe = (const bwag_pe_read_t *)b->d_pe_reads.p;
+	BWAG_LAUNCH(k_pe_text, fm_grid(c, n), 128, 0, c->stream, c->ix, a, d_pe, 0);
+	BWAG_LAUNCH(k_fm_scan64, 1, FM_SCAN_THREADS, 0, c->stream, (const i64 *)b->d_se_tlen.p, (i64)n, (i64 *)b->d_se_tbeg.p, &c->d_cnt->se_total);
+	CK(cudaGetLastError());
+	if (fetch_counters(c)) return 1;
+	c->st.n_launch += 2;
+	c->st.glb_cells += c->h_cnt->se_cells;
+	*n_glb = (int64_t)c->h_cnt->se_run;
+	if (c->h_cnt->se_past) {
+		*past_end = n - c->h_cnt->se_past;
+		return set_err("read %d of the batch: its gapped alignment window runs past the end of the forward strand", *past_end);
+	}
+	const i64 n_text = (i64)c->h_cnt->se_total;
+	if (buf_reserve(&b->d_se_text, (size_t)n_text + 1) || hbuf_reserve(&b->h_se_text, (size_t)n_text + 1)) return 1;
+	a.text = (char *)b->d_se_text.p;
+	BWAG_LAUNCH(k_pe_text, fm_grid(c, n), 128, 0, c->stream, c->ix, a, d_pe, 1);
+	CK(cudaGetLastError());
+	++c->st.n_launch;
+	CK(cudaEventRecord(c->ev0, c->stream));
+	if (n_text) D2H(c, b->h_se_text.p, b->d_se_text.p, (size_t)n_text);
+	D2H(c, b->h_se_rec.p, b->d_se_rec.p, sizeof(bwag_samrec_t) * (size_t)n);
 	CK(cudaEventRecord(c->ev1, c->stream));
 	CK(stream_wait(c));
 	c->st.ms_d2h += elapsed_at(c, "d2h", __LINE__);

@@ -259,6 +259,17 @@ __global__ void k_se_pos(SeArgs a);
 __global__ void k_se_refine(DevIndex ix, SeArgs a);
 __global__ void k_se_text(DevIndex ix, SeArgs a, int write);
 
+/* ---- sampe (bwag_sampe.cu) ---- */
+struct PePosArgs { i64 n, l_pac; const i64 *rows; const int *ref_len; i64 *pos; uint8_t *strand; };   /* [n] rows, [2n] the rest */
+struct PeGlbArgs {
+	int n_tasks; const bwag_pe_gtask_t *tasks; bwag_pe_gres_t *res; u32 *cig; const uint8_t *pool;
+	int *eh; uint8_t *rseq, *z; int cap_q, cap_r; i64 cap_z;   /* per-warp scratch */
+	int *next_task; u64 *cells;
+};
+__global__ void k_pe_pos(PePosArgs a);
+__global__ void k_pe_global(DevIndex ix, PeGlbArgs a);
+__global__ void k_pe_text(DevIndex ix, SeArgs a, const bwag_pe_read_t *pe, int write);
+
 __global__ void k_chain_emit(ChainArgs a);
 __global__ void k_global_lane(DevIndex ix, GlbLaneArgs a);
 __global__ void k_localsw(DevIndex ix, SwArgs a);

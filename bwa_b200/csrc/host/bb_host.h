@@ -195,6 +195,9 @@ void bb_reads_free(bb_reads_t *g);
 /* ---- `bwa-b200 samse` (bb_samse.c) ---- */
 int bb_samse_main(int argc, char *argv[]);
 
+/* ---- `bwa-b200 sampe` (bb_sampe.c) ---- */
+int bb_sampe_main(int argc, char *argv[]);
+
 #ifdef __cplusplus
 }
 #endif

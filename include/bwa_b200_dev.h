@@ -297,6 +297,40 @@ int bwag_ctx_set_ambs(bwag_ctx_t *ctx, int n_holes, const int64_t *offset, const
  * reference aborts on its assert there, bwase.c:180); the call then fails.  n_sa, n_glb: SA rows resolved, global alignments run. */
 int bwag_samse(bwag_batch_t *b, const bwag_samse_par_t *par, bwag_sam_t *out, int *past_end, int64_t *n_sa, int64_t *n_glb);
 
+/* ---- paired-end SAM of `bwa sampe` (bwape.c:260-711, with bwa_print_sam1 of a pair) --------------------------------------------
+ * The host chooses the hits (serial random draws), infers the insert size, pairs and picks XA; the device resolves the suffix-array
+ * rows, runs the mate rescue's alignments and writes the records.  BWAG_UNSUPPORTED from the CPU oracle of the tests.
+ * bwag_pe_sa2pos: n_rows rows, resolved once through the resident suffix array, then bwa_sa2pos with the two reference lengths
+ * ref_len[2k], ref_len[2k + 1] of row k into pos[2k], pos[2k + 1] ((uint64_t)-1: across the strand boundary) and strand[]. */
+int bwag_pe_sa2pos(bwag_batch_t *b, int64_t n_rows, const uint64_t *rows, const int32_t *ref_len, int64_t *pos, uint8_t *strand);
+/* the mate rescue's global alignment (bwa_sw_core, bwape.c:434): ksw_global, scores bwa_fill_scmat(1, 3), gaps 5/1, band 50, of
+ * pool[q_beg, q_beg + qlen) against the forward reference [t_beg, t_beg + tlen); the raw CIGAR (len << 4 | op) at res[i].cig_off of
+ * *cig.  Results pinned, valid until the next call on this batch. */
+typedef struct { int64_t t_beg, q_beg; int32_t tlen, qlen; } bwag_pe_gtask_t;
+typedef struct { int32_t score, n_cigar; int64_t cig_off; } bwag_pe_gres_t;
+int bwag_pe_global(bwag_batch_t *b, int n_tasks, const bwag_pe_gtask_t *tasks, const uint8_t *pool, size_t pool_bytes, const bwag_pe_gres_t **res, const uint32_t **cig);
+/* the pair's records.  reads[2i] and reads[2i + 1] are the two ends of pair i; their type 3 is a mate-rescued hit (BWA_TYPE_MATESW),
+ * whose CIGAR (16-bit entries) the caller gives; the caller's positions are the final ones before the gapped refinement, and its XA
+ * lists hold only the candidates kept (positions in mpos / mstrand). */
+typedef struct {
+	int64_t cig_off; int32_t n_cig;   /* type 3: par->cig[cig_off, cig_off + n_cig) */
+	uint8_t flag;                     /* extra_flag: 0x1, 0x2 (proper pair), 0x40 / 0x80 */
+	uint8_t seq_q;                    /* SM: the single-end mapping quality */
+	uint8_t comp, pad;                /* comp: the read's rseq is complemented (COMPREAD of its own .sai) */
+} bwag_pe_read_t;
+typedef struct {
+	int mode, max_top2;               /* mode: NM (COMPREAD) or CM, from .sai 2 as in the reference */
+	int comp[2];                      /* per end: its rseq complemented (COMPREAD of that end's .sai) */
+	const char *rg_id;
+	const bwag_se_read_t *reads; const bwag_pe_read_t *pe;      /* [n_reads] */
+	const int64_t *pos; const uint8_t *strand;                  /* [n_reads]; an unmapped read's strand is 0 */
+	const bwag_se_hit_t *multi; const int64_t *mpos; const uint8_t *mstrand; int64_t n_multi;
+	const uint32_t *cig; int64_t n_cig;
+	const char *bc; int64_t l_bc;
+} bwag_sampe_par_t;
+/* past_end as bwag_samse; n_glb: gapped refinements run */
+int bwag_sampe(bwag_batch_t *b, const bwag_sampe_par_t *par, bwag_sam_t *out, int *past_end, int64_t *n_glb);
+
 /* ---- work / time counters for the roofline ---------------------------------------------------- */
 typedef struct {
 	uint64_t occ_touches;      /* 64-byte Occ blocks touched by bwt_extend (1 or 2 per call, bwt.c:194-197) */
