@@ -62,6 +62,7 @@ struct Counters {
 	u64 aln_pool, aln_total;
 	u64 se_total, se_run, se_cells;   /* samse: text bytes of the batch (scan total), global alignments run and their cells */
 	int se_next, se_past;             /* samse: next refinement task; n_reads - the first read whose window runs past the forward strand (0: none) */
+	u64 pm_total;                     /* pemerge: text bytes of the batch (scan total) */
 };
 
 struct DevBuf { void *p; size_t cap; };
@@ -157,6 +158,9 @@ struct bwag_batch {
 	/* sampe (bwag_sampe.cu; the rest of its buffers are samse's) */
 	DevBuf d_pe_rlen, d_pe_reads, d_pe_gtasks, d_pe_gres, d_pe_gcig, d_pe_pool;
 	HostBuf h_pe_pos, h_pe_gres, h_pe_gcig;
+	/* pemerge (bwag_pemerge.cu; K6's buffers hold its tasks, codes and alignments) */
+	DevBuf d_pm_qual, d_pm_hasq, d_pm_names, d_pm_noff, d_pm_q, d_pm_code, d_pm_ovl, d_pm_tlen, d_pm_tbeg, d_pm_text, d_pm_cnt;
+	HostBuf h_pm_text, h_pm_cnt;
 	int tail_ready;             /* bwag_tail_regs ran on this batch */
 	int regs_on_device;          /* bwag_chain_extend left the regions in HBM */
 };
@@ -268,6 +272,23 @@ static int pick_grid(bwag_ctx_t *c)
 static cudaEvent_t g_trace_ref;   /* BWA_B200_GPUTRACE: origin of the device-clock timeline (see elapsed_at) */
 static int g_gputrace = -1;
 
+/* what every context owns besides its index: stream, events, counters, launch grids */
+static int ctx_init(bwag_ctx_t *c)
+{
+	CK(cudaStreamCreate(&c->stream));
+	CK(cudaEventCreate(&c->ev0)); CK(cudaEventCreate(&c->ev1));
+	if (g_gputrace < 0) {
+		const char *e = getenv("BWA_B200_GPUTRACE");
+		g_gputrace = e && atoi(e) > 0;
+		if (g_gputrace) { CK(cudaEventCreate(&g_trace_ref)); CK(cudaEventRecord(g_trace_ref, c->stream)); CK(cudaEventSynchronize(g_trace_ref)); }
+	}
+	CK(cudaEventCreateWithFlags(&c->ev_wait, cudaEventBlockingSync | cudaEventDisableTiming));
+	CK(cudaMalloc((void **)&c->d_cnt, sizeof(Counters)));
+	CK(cudaMallocHost((void **)&c->h_cnt, sizeof(Counters)));
+	pthread_mutex_init(&c->mu, 0);
+	return pick_grid(c);
+}
+
 extern "C" bwag_ctx_t *bwag_ctx_from_blob(int device, void *d_blob, int own_blob)
 {
 	BlobHeader h;
@@ -285,6 +306,7 @@ extern "C" bwag_ctx_t *bwag_ctx_from_blob(int device, void *d_blob, int own_blob
 	}
 	bwag_ctx_t *c = (bwag_ctx_t *)calloc(1, sizeof(*c));
 	c->device = device; c->own_blob = own_blob; c->blob = d_blob;
+	if (ctx_init(c)) { free(c); return 0; }
 	char *d = (char *)d_blob;
 	c->ix.bwt = (const uint4 *)(d + h.off_bwt);
 	c->ix.sa = (const u64 *)(d + h.off_sa);
@@ -294,18 +316,19 @@ extern "C" bwag_ctx_t *bwag_ctx_from_blob(int device, void *d_blob, int own_blob
 	for (int s = 0; s < BWAG_MAX_SB; ++s)
 		for (int k = 0; k < 4; ++k) { c->ix.sb[s][k] = h.sb[s][k]; c->ix.sbgt[s][k] = 0; for (int t = k + 1; t < 4; ++t) c->ix.sbgt[s][k] += h.sb[s][t]; }
 	c->sa_intv_disk = 1 << h.sa_shift;
-	CKP(cudaStreamCreate(&c->stream));
-	CKP(cudaEventCreate(&c->ev0)); CKP(cudaEventCreate(&c->ev1));
-	if (g_gputrace < 0) {
-		const char *e = getenv("BWA_B200_GPUTRACE");
-		g_gputrace = e && atoi(e) > 0;
-		if (g_gputrace) { CKP(cudaEventCreate(&g_trace_ref)); CKP(cudaEventRecord(g_trace_ref, c->stream)); CKP(cudaEventSynchronize(g_trace_ref)); }
-	}
-	CKP(cudaEventCreateWithFlags(&c->ev_wait, cudaEventBlockingSync | cudaEventDisableTiming));
-	CKP(cudaMalloc((void **)&c->d_cnt, sizeof(Counters)));
-	CKP(cudaMallocHost((void **)&c->h_cnt, sizeof(Counters)));
-	pthread_mutex_init(&c->mu, 0);
-	if (pick_grid(c)) { free(c); return 0; }
+	return c;
+}
+
+/* a context without an index (pemerge): the index view stays zeroed, which K6 reads only for targets on the reference */
+extern "C" bwag_ctx_t *bwag_ctx_create_bare(int device)
+{
+	int ndev = 0;
+	if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { set_err("no CUDA device is visible: this library has no CPU path"); return 0; }
+	if (device < 0) CKP(cudaGetDevice(&device));
+	CKP(cudaSetDevice(device));
+	bwag_ctx_t *c = (bwag_ctx_t *)calloc(1, sizeof(*c));
+	c->device = device;
+	if (ctx_init(c)) { free(c); return 0; }
 	return c;
 }
 
@@ -722,6 +745,8 @@ static void batch_free(bwag_batch_t *b)
 	free_dev(&b->d_se_rec); free_dev(&b->d_se_text); free_dev(&b->d_se_nm); free_host(&b->h_se_tasks); free_host(&b->h_se_mtask); free_host(&b->h_se_rec); free_host(&b->h_se_text);
 	free_dev(&b->d_pe_rlen); free_dev(&b->d_pe_reads); free_dev(&b->d_pe_gtasks); free_dev(&b->d_pe_gres); free_dev(&b->d_pe_gcig); free_dev(&b->d_pe_pool);
 	free_host(&b->h_pe_pos); free_host(&b->h_pe_gres); free_host(&b->h_pe_gcig);
+	free_dev(&b->d_pm_qual); free_dev(&b->d_pm_hasq); free_dev(&b->d_pm_names); free_dev(&b->d_pm_noff); free_dev(&b->d_pm_q); free_dev(&b->d_pm_code); free_dev(&b->d_pm_ovl);
+	free_dev(&b->d_pm_tlen); free_dev(&b->d_pm_tbeg); free_dev(&b->d_pm_text); free_dev(&b->d_pm_cnt); free_host(&b->h_pm_text); free_host(&b->h_pm_cnt);
 	free(b);
 }
 
@@ -1757,6 +1782,81 @@ extern "C" int bwag_localsw(bwag_batch_t *b, const bwag_sw_par_t *par, int n_tas
 	c->st.ms_localsw += elapsed_at(c, "localsw", __LINE__); ++c->st.n_launch; c->st.sw_tasks += (u64)n_tasks;
 	if (c->h_cnt->flags & 32u) return set_err("local alignment: a task exceeded the scratch capacity");
 	*out = (const bwag_swres_t *)b->h_swres.p;
+	return 0;
+}
+
+/* ------------------------------------------------------------------------------------------------ pemerge */
+
+/* M1, K6, M2/M3, then M4 around a scan (bwag_pemerge.cu) */
+extern "C" int bwag_pemerge(bwag_batch_t *b, const bwag_pemerge_par_t *par, bwag_pemerge_t *out)
+{
+	bwag_ctx_t *c = &b->lc;
+	CK(cudaSetDevice(c->device));
+	memset(out, 0, sizeof(*out));
+	const int n = b->n;
+	if (n & 1) return set_err("bwag_pemerge: a batch of %d reads is not a batch of pairs", n);
+	const int np = n >> 1;
+	const i64 nb = b->total_bases, nn = par->name_off[n];
+	int max_q = 16, max_t = 16;
+	for (int i = 0; i < np; ++i) {
+		const int l0 = (int)(b->h_off[2 * i + 1] - b->h_off[2 * i]), l1 = (int)(b->h_off[2 * i + 2] - b->h_off[2 * i + 1]);
+		if (l0 > max_t) max_t = l0;
+		if (l1 > max_q) max_q = l1;
+	}
+	if (buf_reserve(&b->d_pm_qual, (size_t)nb + 16) || buf_reserve(&b->d_pm_hasq, (size_t)n + 16) || buf_reserve(&b->d_pm_names, (size_t)nn + 16) ||
+	    buf_reserve(&b->d_pm_noff, 8 * ((size_t)n + 1)) || buf_reserve(&b->d_swpool, (size_t)nb + 16) || buf_reserve(&b->d_pm_q, (size_t)nb + 16) ||
+	    buf_reserve(&b->d_swtasks, sizeof(bwag_swtask_t) * ((size_t)np + 1)) || buf_reserve(&b->d_pm_code, (size_t)np + 16) || buf_reserve(&b->d_pm_ovl, 4 * ((size_t)np + 1)) ||
+	    buf_reserve(&b->d_pm_tlen, 8 * ((size_t)np + 1)) || buf_reserve(&b->d_pm_tbeg, 8 * ((size_t)np + 1)) || buf_reserve(&b->d_pm_cnt, 8 * 9) ||
+	    hbuf_reserve(&b->h_pm_cnt, 8 * 9)) return 1;
+	PemArgs a;
+	memset(&a, 0, sizeof(a));
+	a.n_pairs = np; a.T = par->T; a.q_thres = par->q_thres; a.q_def = par->q_def; a.flag = par->flag;
+	a.raw = (const uint8_t *)b->d_codes.p; a.off = (const i64 *)b->d_off.p;
+	a.qual = (const uint8_t *)b->d_pm_qual.p; a.has_qual = (const uint8_t *)b->d_pm_hasq.p;
+	a.names = (const char *)b->d_pm_names.p; a.name_off = (const i64 *)b->d_pm_noff.p;
+	a.s = (uint8_t *)b->d_swpool.p; a.q = (uint8_t *)b->d_pm_q.p; a.tasks = (bwag_swtask_t *)b->d_swtasks.p;
+	a.code = (int8_t *)b->d_pm_code.p; a.ovl = (int *)b->d_pm_ovl.p;
+	a.tlen = (i64 *)b->d_pm_tlen.p; a.tbeg = (const i64 *)b->d_pm_tbeg.p; a.cnt = (u64 *)b->d_pm_cnt.p;
+	if (reset_counters(c)) return 1;
+	if (nb) H2D(c, b->d_pm_qual.p, par->qual, (size_t)nb);
+	if (n) H2D(c, b->d_pm_hasq.p, par->has_qual, (size_t)n);
+	if (nn) H2D(c, b->d_pm_names.p, par->names, (size_t)nn);
+	H2D(c, b->d_pm_noff.p, par->name_off, 8 * ((size_t)n + 1));
+	CK(cudaMemsetAsync(b->d_pm_cnt.p, 0, 8 * 9, c->stream));
+	if (np) BWAG_LAUNCH(k_pem_encode, fm_grid(c, np), 128, 0, c->stream, a);
+	CK(cudaGetLastError());
+	++c->st.n_launch;
+	if (par->merge && np) {
+		bwag_sw_par_t sp;   /* ksw_align(l2, s1, l1, s0, 5, bwa_fill_scmat(5, 4), 2, 17, xtra): the same gaps for deletions and insertions */
+		memset(&sp, 0, sizeof(sp));
+		sp.a = 5; sp.b = 4; sp.o_del = sp.o_ins = 2; sp.e_del = sp.e_ins = 17;
+		for (int i = 0; i < 5; ++i) for (int j = 0; j < 5; ++j) sp.mat[i * 5 + j] = (int8_t)(i < 4 && j < 4 ? (i == j ? 5 : -4) : -1);
+		if (localsw_on_device(b, &sp, np, max_q, max_t)) return 1;
+		a.res = (const bwag_swres_t *)b->d_swres.p;
+		const i64 blocks = ((i64)np + 3) / 4, cap = (i64)c->n_sm * 16;
+		BWAG_LAUNCH(k_pem_decide, (int)(blocks < cap ? blocks : cap), 128, 0, c->stream, a);
+		CK(cudaGetLastError());
+		if (fetch_counters(c)) return 1;
+		c->st.ms_localsw += elapsed_at(c, "localsw", __LINE__); c->st.n_launch += 2; c->st.sw_tasks += (u64)np;
+		if (c->h_cnt->flags & 32u) return set_err("pemerge: a local alignment exceeded the scratch capacity");
+	}
+	/* M4: sizes, their scan, then the text */
+	if (np) BWAG_LAUNCH(k_pem_text, fm_grid(c, np), 128, 0, c->stream, a, 0);
+	BWAG_LAUNCH(k_fm_scan64, 1, FM_SCAN_THREADS, 0, c->stream, (const i64 *)b->d_pm_tlen.p, (i64)np, (i64 *)b->d_pm_tbeg.p, &c->d_cnt->pm_total);
+	CK(cudaGetLastError());
+	if (fetch_counters(c)) return 1;
+	c->st.n_launch += 2;
+	const i64 n_text = (i64)c->h_cnt->pm_total;
+	if (buf_reserve(&b->d_pm_text, (size_t)n_text + 16) || hbuf_reserve(&b->h_pm_text, (size_t)n_text + 16)) return 1;
+	a.text = (char *)b->d_pm_text.p;
+	if (np) BWAG_LAUNCH(k_pem_text, fm_grid(c, np), 128, 0, c->stream, a, 1);
+	CK(cudaGetLastError());
+	++c->st.n_launch;
+	if (n_text) D2H(c, b->h_pm_text.p, b->d_pm_text.p, (size_t)n_text);
+	D2H(c, b->h_pm_cnt.p, b->d_pm_cnt.p, 8 * 9);
+	CK(stream_wait(c));
+	out->text = (const char *)b->h_pm_text.p; out->n_text = n_text;
+	memcpy(out->cnt, b->h_pm_cnt.p, 8 * 9);
 	return 0;
 }
 

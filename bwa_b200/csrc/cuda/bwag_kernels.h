@@ -270,6 +270,22 @@ __global__ void k_pe_pos(PePosArgs a);
 __global__ void k_pe_global(DevIndex ix, PeGlbArgs a);
 __global__ void k_pe_text(DevIndex ix, SeArgs a, const bwag_pe_read_t *pe, int write);
 
+/* ---- pemerge (bwag_pemerge.cu) ---- */
+struct PemArgs {
+	int n_pairs, T, q_thres, q_def, flag;
+	const uint8_t *raw; const i64 *off;              /* the batch: raw sequence bytes; read 1 of pair i is read 2i, read 2 is read 2i + 1 */
+	const uint8_t *qual; const uint8_t *has_qual;    /* raw quality bytes at the reads' offsets; per read: it has a quality string */
+	const char *names; const i64 *name_off;          /* [2 n_pairs + 1] */
+	uint8_t *s, *q;                                  /* codes (K6's pool) and qualities - 33: s0 / q0 at read 1's offset, s1 / q1 at read 2's */
+	bwag_swtask_t *tasks; const bwag_swres_t *res;   /* K6: task i is pair i */
+	int8_t *code; int *ovl;                          /* [n_pairs] 0 merged, -1 .. -8 why not, 1 not tried; the overlap of a merge */
+	i64 *tlen; const i64 *tbeg; char *text;          /* the records: bytes per pair, their scan, the text */
+	u64 *cnt;                                        /* [9] pairs per outcome */
+};
+__global__ void k_pem_encode(PemArgs a);
+__global__ void k_pem_decide(PemArgs a);
+__global__ void k_pem_text(PemArgs a, int write);
+
 __global__ void k_chain_emit(ChainArgs a);
 __global__ void k_global_lane(DevIndex ix, GlbLaneArgs a);
 __global__ void k_localsw(DevIndex ix, SwArgs a);

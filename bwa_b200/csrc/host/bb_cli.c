@@ -470,6 +470,7 @@ int main(int argc, char *argv[])
 	if (argc >= 2 && strcmp(argv[1], "aln") == 0) { free(pg.s); ret = bb_aln_main(argc - 1, argv + 1); fflush(stdout); return ret; }
 	if (argc >= 2 && strcmp(argv[1], "samse") == 0) { ret = bb_samse_main(argc - 1, argv + 1); fflush(stdout); free(pg.s); return ret; }
 	if (argc >= 2 && strcmp(argv[1], "sampe") == 0) { ret = bb_sampe_main(argc - 1, argv + 1); fflush(stdout); free(pg.s); return ret; }
+	if (argc >= 2 && strcmp(argv[1], "pemerge") == 0) { free(pg.s); ret = bb_pemerge_main(argc - 1, argv + 1); fflush(stdout); return ret; }
 	if (argc < 2 || strcmp(argv[1], "mem") != 0) {
 		fprintf(stderr, "\nProgram: bwa-b200 (BWA-MEM seed-and-extend on NVIDIA H100)\nVersion: %s\n\nUsage:   bwa-b200 index [-p prefix] <in.fasta[.gz]>   build the index files on the GPU\n", BB_VERSION);
 		fprintf(stderr, "         bwa-b200 mem [options] <idxbase> <in1.fq> [in2.fq]\n");
@@ -478,6 +479,7 @@ int main(int argc, char *argv[])
 		fprintf(stderr, "         bwa-b200 samse [-n max_occ] [-f out.sam] [-r RG_line] <idxbase> <in.sai> <in.fq>   single-end SAM from a .sai file\n");
 		fprintf(stderr, "         bwa-b200 sampe [-a maxins] [-o maxocc] [-n INT] [-N INT] [-c FLOAT] [-f out.sam] [-r RG_line] [-P] [-s] [-A]\n"
 		                "                        <idxbase> <in1.sai> <in2.sai> <in1.fq> <in2.fq>   paired-end SAM from two .sai files\n");
+		fprintf(stderr, "         bwa-b200 pemerge [-mu] [-t INT] [-T INT] [-Q INT] <read1.fq> [read2.fq]   merge overlapping read pairs\n");
 		fprintf(stderr, "         bwa-b200 shm [-d|-l] [idxbase]      keep an index resident on the GPU between runs\n\nThe index is the one `bwa index` writes; `bwa-b200 index` writes the same files.\n\n");
 		return 1;
 	}

@@ -198,6 +198,9 @@ int bb_samse_main(int argc, char *argv[]);
 /* ---- `bwa-b200 sampe` (bb_sampe.c) ---- */
 int bb_sampe_main(int argc, char *argv[]);
 
+/* ---- `bwa-b200 pemerge` (bb_pemerge.c) ---- */
+int bb_pemerge_main(int argc, char *argv[]);
+
 #ifdef __cplusplus
 }
 #endif

@@ -331,6 +331,28 @@ typedef struct {
 /* past_end as bwag_samse; n_glb: gapped refinements run */
 int bwag_sampe(bwag_batch_t *b, const bwag_sampe_par_t *par, bwag_sam_t *out, int *past_end, int64_t *n_glb);
 
+/* ---- read-pair merging of `bwa pemerge` (bwa_pemerge and the printing loop, pemerge.c:59-215) ------------------------------------
+ * No index is involved: the batch comes from a context made by bwag_ctx_create_bare (a stream and buffers, no index), and its "codes"
+ * are the reads' raw sequence bytes, read 1 of pair i as read 2i and read 2 as read 2i + 1.  Per pair, on the device: the codes and
+ * qualities, the local alignment of read 2's reverse complement against read 1 (K6: ksw_align with KSW_XSTART | KSW_XSUBO, scores
+ * bwa_fill_scmat(5, 4), gaps 2/17), the reference's eight tests in its order, the merged read and the records print_bseq writes,
+ * whole (names included), in pair order.  cnt[k]: pairs whose bwa_pemerge returned -k.  BWAG_UNSUPPORTED from the CPU oracle of the
+ * tests. */
+bwag_ctx_t *bwag_ctx_create_bare(int device);   /* device < 0: the current one; NULL (bwag_last_error says why) without a device */
+typedef struct {
+	int T;                       /* minimum score: 5 x the minimum overlap (-T) */
+	int q_thres;                 /* -Q */
+	int q_def;                   /* the quality of every base of a read without qualities (20) */
+	int flag;                    /* 1: print merged pairs, 2: unmerged ones */
+	int merge;                   /* 0: try no pair (the reference with -t 0): every count 0, every pair printed as it came */
+	const uint8_t *qual;         /* raw quality bytes at the offsets of the batch's reads (any bytes where has_qual is 0) */
+	const uint8_t *has_qual;     /* [n_reads] the read has a quality string (a FASTQ read that is not empty) */
+	const char *names;           /* the reads' names after trim_readno, back to back */
+	const int64_t *name_off;     /* [n_reads + 1] */
+} bwag_pemerge_par_t;
+typedef struct { const char *text; int64_t n_text; int64_t cnt[9]; } bwag_pemerge_t;   /* text: pinned, valid until the next call on the batch */
+int bwag_pemerge(bwag_batch_t *b, const bwag_pemerge_par_t *par, bwag_pemerge_t *out);
+
 /* ---- work / time counters for the roofline ---------------------------------------------------- */
 typedef struct {
 	uint64_t occ_touches;      /* 64-byte Occ blocks touched by bwt_extend (1 or 2 per call, bwt.c:194-197) */
