@@ -1,16 +1,14 @@
 /* bb_aln.c -- `bwa-b200 aln`: BWA-backtrack, the .sai stream of the reference's `bwa aln` (bwtaln.c:159-321) byte for byte, with the
  * search on the GPU (bwag_aln, bwag_aln.cu).  `bwa samse` / `bwa sampe` read what it writes.
  *
- * Three threads overlap: a reader parses the reads as bwa_read_seq does (bb_read_group, bb_seqio.c) in the reference's groups of
- * 262144 reads and cuts each group into device batches of BWA_B200_ALN_CHUNK reads; the calling thread runs the current batch on
- * the device; a writer prints the previous one.  Batches pass through single-slot mailboxes, so the output keeps the input order and at most four batches exist at a time.
- * The group matters: the reference clamps max_gapo to the max_diff of the group's longest read (bwtaln.c:91-94), and that value
- * enters every search of the group.  max_diff itself (bwa_cal_maxdiff, a libm expression) is computed here, per read, and handed
+ * It runs on the pipeline of bb_util.h: the reader parses the reads as bwa_read_seq does (bb_read_group, bb_seqio.c) in the
+ * reference's groups of 262144 reads and cuts each group into device batches of BWA_B200_ALN_CHUNK reads.  The group matters: the
+ * reference clamps max_gapo to the max_diff of the group's longest read (bwtaln.c:91-94), and that value enters every search of the
+ * group.  max_diff itself (bwa_cal_maxdiff, a libm expression) is computed here, per read, and handed
  * to the device.  BWA_B200_PROFILE=1 reports the index load, the busy time of the three threads and the reads of tier 2. */
 #include <unistd.h>
 #include <math.h>
 #include <stddef.h>
-#include <pthread.h>
 #include "bb_host.h"
 
 #define ALN_MAX_LEN   65536      /* the reference keeps a read's remaining length in 16 bits of its queue entries (bwtgap.c:61,142) */
@@ -44,8 +42,10 @@ typedef struct {
 	const aln_opt_t *opt;
 	int chunk;
 	int *md_of_len;            /* [ALN_MAX_LEN] max_diff by read length (-1: not computed yet) */
-	bb_mbox_t to_dev, to_write;
-	double t_read, t_write;
+	bwag_ctx_t *ctx;
+	bwag_aln_par_t par;
+	long long n_tier2;
+	int header_out;            /* writer: the .sai header is out */
 } aln_run_t;
 
 static int read_maxdiff(aln_run_t *r, int len)
@@ -106,61 +106,58 @@ static aln_batch_t *slice(const aln_batch_t *g, int beg, int end)
 	return b;
 }
 
-static void *reader_main(void *arg)
+static void read_all(bb_pipe_t *p, void *run)
 {
-	aln_run_t *r = arg;
-	for (;;) {
-		double t0 = bb_realtime();
-		aln_batch_t *g = read_group(r);
-		r->t_read += bb_realtime() - t0;
-		if (!g) break;
-		if (g->n <= r->chunk) { bb_mbox_put(&r->to_dev, g); continue; }
-		for (int beg = 0; beg < g->n; beg += r->chunk) {
-			const int end = beg + r->chunk < g->n ? beg + r->chunk : g->n;
-			t0 = bb_realtime();
-			aln_batch_t *b = slice(g, beg, end);
-			r->t_read += bb_realtime() - t0;
-			bb_mbox_put(&r->to_dev, b);
-		}
+	aln_run_t *r = run;
+	aln_batch_t *g;
+	while ((g = read_group(r)) != 0) {
+		if (g->n <= r->chunk) { bb_pipe_to_device(p, g); continue; }
+		for (int beg = 0; beg < g->n; beg += r->chunk) bb_pipe_to_device(p, slice(g, beg, beg + r->chunk < g->n ? beg + r->chunk : g->n));
 		batch_free(g);
 	}
-	bb_mbox_put(&r->to_dev, 0);
-	return 0;
+}
+
+static void run_device(bb_pipe_t *p, void *run, void *item)
+{
+	aln_run_t *r = run;
+	aln_batch_t *b = item;
+	int rc;
+	if ((b->dev = bwag_batch_begin(r->ctx, b->n, b->codes, b->off)) == 0) bb_fatal("bwa_aln", "cannot start a device batch: %s", bwag_last_error());
+	r->par.max_gapo = b->max_gapo; r->par.max_diff = b->md;
+	rc = bwag_aln(b->dev, &r->par, &b->res);
+	if (rc == BWAG_UNSUPPORTED) { fprintf(stderr, "[E::%s] this build has no device backtracking search\n", "bwa_aln"); exit(1); }
+	if (rc != 0) bb_fatal("bwa_aln", "device search failed: %s", bwag_last_error());
+	r->n_tier2 += b->res.n_tier2;
+	bb_pipe_to_writer(p, b);
+}
+
+/* the header goes out once the first batch has been searched (or the input turned out empty): a build without the device search
+ * leaves stdout empty */
+static void write_header(aln_run_t *r)
+{
+	if (fwrite("SAI\1", 1, 4, stdout) != 4 || fwrite(r->opt, sizeof(*r->opt), 1, stdout) != 1) bb_fatal("bwa_aln", "fail to write the output");
+	r->header_out = 1;
 }
 
 /* per read: int32 n_aln, then its n_aln 24-byte records (bwtaln.c:214-218) */
-static void write_batch(const aln_batch_t *b)
+static void write_batch(void *run, void *item)
 {
+	aln_run_t *r = run;
+	aln_batch_t *b = item;
 	bb_str_t s = {0, 0, 0};
 	int i;
+	if (!r->header_out) write_header(r);
 	for (i = 0; i < b->n; ++i) {
 		const int32_t n = b->res.n_aln[i];
 		bb_putsn(&s, (const char *)&n, 4);
 		if (n) bb_putsn(&s, (const char *)(b->res.aln + b->res.off[i]), sizeof(bwag_aln1_t) * (size_t)n);
-		if (s.l >= (1 << 20)) {
-			if (fwrite(s.s, 1, s.l, stdout) != s.l) bb_fatal("bwa_aln", "fail to write the output");
-			s.l = 0;
-		}
+		bb_str_write(&s, 1 << 20, "bwa_aln");
 	}
-	if (s.l && fwrite(s.s, 1, s.l, stdout) != s.l) bb_fatal("bwa_aln", "fail to write the output");
-	free(s.s);
+	bb_str_write(&s, 0, "bwa_aln");
+	batch_free(b);   /* the device batch too: its pinned buffers held the hits until now */
 }
 
-static void *writer_main(void *arg)
-{
-	aln_run_t *r = arg;
-	aln_batch_t *b = bb_mbox_get(&r->to_write);
-	/* the header goes out once the first batch has been searched (or the input turned out empty): a build without the device
-	 * search leaves stdout empty */
-	if (fwrite("SAI\1", 1, 4, stdout) != 4 || fwrite(r->opt, sizeof(*r->opt), 1, stdout) != 1) bb_fatal("bwa_aln", "fail to write the output");
-	for (; b != 0; b = bb_mbox_get(&r->to_write)) {
-		double t0 = bb_realtime();
-		write_batch(b);
-		batch_free(b);   /* the device batch too: its pinned buffers held the hits until now */
-		r->t_write += bb_realtime() - t0;
-	}
-	return 0;
-}
+static const bb_pipe_ops_t ops = { read_all, run_device, write_batch };
 
 static void usage(const aln_opt_t *opt)
 {
@@ -196,12 +193,10 @@ int bb_aln_main(int argc, char *argv[])
 	int c, opte = -1;
 	aln_opt_t opt;
 	bwaidx_t *idx;
-	bwag_ctx_t *ctx;
 	aln_run_t run;
-	bwag_aln_par_t par;
-	pthread_t th_r, th_w;
-	double t0, t_load, t_dev = 0;
-	long long n_tier2 = 0;
+	bwag_aln_par_t *par = &run.par;
+	bb_pipe_busy_t busy;
+	double t0, t_load;
 	const char *e;
 
 	memset(&opt, 0, sizeof(opt));   /* gap_init_opt (bwtaln.c:24-40) */
@@ -274,38 +269,18 @@ int bb_aln_main(int argc, char *argv[])
 		bb_fq_close(run.fq); free(run.md_of_len);
 		return 1;
 	}
-	ctx = bb_device_attach(idx->bwt, idx->bns, idx->pac);   /* fails here, before any output, if there is no GPU */
+	run.ctx = bb_device_attach(idx->bwt, idx->bns, idx->pac);   /* fails here, before any output, if there is no GPU */
 	t_load = bb_realtime() - t0;
-	memset(&par, 0, sizeof(par));
-	par.s_mm = opt.s_mm; par.s_gapo = opt.s_gapo; par.s_gape = opt.s_gape;
-	par.mode = opt.mode & (BWAG_ALN_GAPE | BWAG_ALN_LOGGAP | BWAG_ALN_NONSTOP);
-	par.indel_end_skip = opt.indel_end_skip; par.max_del_occ = opt.max_del_occ; par.max_entries = opt.max_entries;
-	par.max_gape = opt.max_gape; par.max_seed_diff = opt.max_seed_diff; par.seed_len = opt.seed_len; par.max_top2 = opt.max_top2;
-
-	bb_mbox_init(&run.to_dev); bb_mbox_init(&run.to_write);
-	pthread_create(&th_r, 0, reader_main, &run);
-	pthread_create(&th_w, 0, writer_main, &run);
-	for (;;) {
-		aln_batch_t *b = bb_mbox_get(&run.to_dev);
-		double t1 = bb_realtime();
-		int rc;
-		if (!b) break;
-		if ((b->dev = bwag_batch_begin(ctx, b->n, b->codes, b->off)) == 0) bb_fatal("bwa_aln", "cannot start a device batch: %s", bwag_last_error());
-		par.max_gapo = b->max_gapo; par.max_diff = b->md;
-		rc = bwag_aln(b->dev, &par, &b->res);
-		if (rc == BWAG_UNSUPPORTED) { fprintf(stderr, "[E::%s] this build has no device backtracking search\n", "bwa_aln"); exit(1); }
-		if (rc != 0) bb_fatal("bwa_aln", "device search failed: %s", bwag_last_error());
-		n_tier2 += b->res.n_tier2;
-		t_dev += bb_realtime() - t1;
-		bb_mbox_put(&run.to_write, b);
-	}
-	bb_mbox_put(&run.to_write, 0);
-	pthread_join(th_r, 0);
-	pthread_join(th_w, 0);
+	par->s_mm = opt.s_mm; par->s_gapo = opt.s_gapo; par->s_gape = opt.s_gape;
+	par->mode = opt.mode & (BWAG_ALN_GAPE | BWAG_ALN_LOGGAP | BWAG_ALN_NONSTOP);
+	par->indel_end_skip = opt.indel_end_skip; par->max_del_occ = opt.max_del_occ; par->max_entries = opt.max_entries;
+	par->max_gape = opt.max_gape; par->max_seed_diff = opt.max_seed_diff; par->seed_len = opt.seed_len; par->max_top2 = opt.max_top2;
+	bb_pipe_run(&ops, &run, &busy);
+	if (!run.header_out) write_header(&run);   /* an empty input */
 	if (fflush(stdout) != 0 || ferror(stdout)) bb_fatal("bwa_aln", "fail to write the output");
 	if (getenv("BWA_B200_PROFILE"))
 		fprintf(stderr, "[prof] aln: index load %.3f s; busy time of the reader %.3f s, the device %.3f s, the writer %.3f s; %lld reads in tier 2; total %.3f s\n",
-		        t_load, run.t_read, t_dev, run.t_write, n_tier2, bb_realtime() - t0);
+		        t_load, busy.read, busy.device, busy.write, run.n_tier2, bb_realtime() - t0);
 	bb_fq_close(run.fq);
 	free(run.md_of_len);
 	bwa_idx_destroy(idx);

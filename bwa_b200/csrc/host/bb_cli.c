@@ -16,34 +16,6 @@
 
 typedef struct { int n; bseq1_t *seqs; int last; int skip; long no, seq_no; int64_t n_before; } batch_t;   /* skip: another rank's batch (multi-GPU runs); no: number in the whole run; seq_no: number in this process (the writer's order) */
 
-typedef struct { /* single-slot mailbox */
-	pthread_mutex_t mu;
-	pthread_cond_t cv;
-	batch_t *slot;
-	int closed;
-} mbox_t;
-
-static void mbox_init(mbox_t *m) { pthread_mutex_init(&m->mu, 0); pthread_cond_init(&m->cv, 0); m->slot = 0; m->closed = 0; }
-static void mbox_put(mbox_t *m, batch_t *b)
-{
-	pthread_mutex_lock(&m->mu);
-	while (m->slot) pthread_cond_wait(&m->cv, &m->mu);
-	m->slot = b;
-	if (!b) m->closed = 1;
-	pthread_cond_broadcast(&m->cv);
-	pthread_mutex_unlock(&m->mu);
-}
-static batch_t *mbox_get(mbox_t *m)
-{
-	batch_t *b;
-	pthread_mutex_lock(&m->mu);
-	while (!m->slot && !m->closed) pthread_cond_wait(&m->cv, &m->mu);
-	b = m->slot; m->slot = 0;
-	pthread_cond_broadcast(&m->cv);
-	pthread_mutex_unlock(&m->mu);
-	return b;
-}
-
 /* finished batches wait here until it is their turn to be written (several batches are aligned at a time) */
 #define RO_SLOTS 8
 typedef struct {
@@ -81,7 +53,7 @@ typedef struct {
 	bwaidx_t *idx;
 	int copy_comment, chunk;
 	int64_t n_processed;
-	mbox_t to_align;
+	bb_mbox_t to_align;   /* closed at the end of the input: every aligner thread then stops */
 	reorder_t done;
 	/* multi-GPU runs (bwa_b200/multi.py): batches are dealt round-robin, batch b belongs to rank b % world; every rank
 	 * parses the whole input so that batch boundaries -- and with them the per-batch insert-size model -- are those of
@@ -146,22 +118,22 @@ static void *reader_main(void *a)
 		int i;
 		int64_t size = 0;
 		if (g_plan_n >= 0) {   /* only this process's batches, each from its byte range; the writer sees just those */
-			if (k >= g_plan_n) { free(b); ro_finish(&r->done, k); mbox_put(&r->to_align, 0); return 0; }
+			if (k >= g_plan_n) { free(b); ro_finish(&r->done, k); bb_mbox_put(&r->to_align, 0); return 0; }
 			b->seqs = read_planned(r, &g_plan[k], &b->n);
 			b->no = g_plan[k].no; b->n_before = g_plan[k].n_before; b->seq_no = k++;
 			if (!b->seqs) bb_fatal("main_mem", "planned batch %ld is empty", b->no);
 		} else {
 			b->seqs = bseq_read(r->chunk, &b->n, r->f1, r->f2);
-			if (!b->seqs) { free(b); ro_finish(&r->done, r->n_batches); mbox_put(&r->to_align, 0); return 0; }
+			if (!b->seqs) { free(b); ro_finish(&r->done, r->n_batches); bb_mbox_put(&r->to_align, 0); return 0; }
 			b->no = b->seq_no = r->n_batches++;
 			b->n_before = r->n_processed; r->n_processed += b->n;
 		}
-		if (g_plan_n < 0 && b->no % r->world != r->rank) { b->skip = 1; free_reads(b); mbox_put(&r->to_align, b); continue; }
+		if (g_plan_n < 0 && b->no % r->world != r->rank) { b->skip = 1; free_reads(b); bb_mbox_put(&r->to_align, b); continue; }
 		if (!r->copy_comment)
 			for (i = 0; i < b->n; ++i) { free(b->seqs[i].comment); b->seqs[i].comment = 0; }
 		for (i = 0; i < b->n; ++i) size += b->seqs[i].l_seq;
 		if (bwa_verbose >= 3) fprintf(stderr, "[M::%s] read %d sequences (%ld bp)...\n", "process", b->n, (long)size);
-		mbox_put(&r->to_align, b);
+		bb_mbox_put(&r->to_align, b);
 	}
 }
 
@@ -205,7 +177,7 @@ static void *aligner_main(void *a)
 {
 	run_t *r = a;
 	batch_t *b;
-	while ((b = mbox_get(&r->to_align)) != 0) {
+	while ((b = bb_mbox_get(&r->to_align)) != 0) {
 		align_batch(r, b);
 		ro_post(&r->done, b);
 	}
@@ -404,7 +376,7 @@ int main_mem(int argc, char *argv[])
 	 * the output is `bwa mem`'s), but the host phases between the GPU stages use the CPUs the process is allowed. */
 	if (!t_given) opt->n_threads = bb_effective_cpus();
 
-	mbox_init(&run.to_align); ro_init(&run.done);
+	bb_mbox_init(&run.to_align); ro_init(&run.done);
 	if (no_mt_io) {
 		int64_t k = 0;
 		for (;;) {

@@ -2,12 +2,10 @@
  * what the reference's `bwa fastmap` prints (fastmap.c:408-483), with the SMEM search, the suffix-array lookups and the EM lines
  * on the GPU (bwag_fastmap: K1 in its fastmap form, K2, bwag_fastmap.cu).
  *
- * Three threads overlap: a reader parses the next batch of reads (BWA_B200_FASTMAP_CHUNK bases, kseq grammar: FASTA/FASTQ, plain or
- * gzip, '-' for stdin), the calling thread runs the current one on the device, and a writer prints the previous one -- per read
- * its SQ line, the device's EM lines and "//".  Batches pass through single-slot mailboxes, so output order is input order and at
- * most four batches exist at a time.  BWA_B200_PROFILE=1 reports the busy time of each of the three and of the index load. */
+ * It runs on the pipeline of bb_util.h: the reader parses batches of BWA_B200_FASTMAP_CHUNK bases (kseq grammar: FASTA/FASTQ, plain
+ * or gzip, '-' for stdin), and the writer prints per read its SQ line, the device's EM lines and "//".  At most four batches exist
+ * at a time.  BWA_B200_PROFILE=1 reports the busy time of the three threads and the index load. */
 #include <unistd.h>
-#include <pthread.h>
 #include "bb_host.h"
 
 #define FM_MAX_LEN (1 << 23)   /* K1 keeps match ends in 23 bits (bwag_smem.cu) */
@@ -27,8 +25,8 @@ typedef struct {
 	bb_fq_t *fq;
 	int64_t chunk;
 	int print_seq;
-	bb_mbox_t to_dev, to_write;
-	double t_read, t_write;
+	bwag_ctx_t *ctx;
+	bwag_fastmap_par_t par;
 } fm_run_t;
 
 static void batch_free(fm_batch_t *b)
@@ -69,20 +67,28 @@ static fm_batch_t *read_batch(fm_run_t *r)
 	return b;
 }
 
-static void *reader_main(void *arg)
+static void read_all(bb_pipe_t *p, void *run)
 {
-	fm_run_t *r = arg;
-	for (;;) {
-		double t0 = bb_realtime();
-		fm_batch_t *b = read_batch(r);
-		r->t_read += bb_realtime() - t0;
-		bb_mbox_put(&r->to_dev, b);
-		if (!b) return 0;
-	}
+	fm_batch_t *b;
+	while ((b = read_batch(run)) != 0) bb_pipe_to_device(p, b);
 }
 
-static void write_batch(const fm_run_t *r, const fm_batch_t *b)
+static void run_device(bb_pipe_t *p, void *run, void *item)
 {
+	fm_run_t *r = run;
+	fm_batch_t *b = item;
+	int rc;
+	if ((b->dev = bwag_batch_begin(r->ctx, b->n, b->codes, b->off)) == 0) bb_fatal("main_fastmap", "cannot start a device batch: %s", bwag_last_error());
+	rc = bwag_fastmap(b->dev, &r->par, &b->res);
+	if (rc == BWAG_UNSUPPORTED) { fprintf(stderr, "[E::%s] this build has no device SMEM lister\n", "main_fastmap"); exit(1); }
+	if (rc != 0) bb_fatal("main_fastmap", "device SMEM listing failed: %s", bwag_last_error());
+	bb_pipe_to_writer(p, b);
+}
+
+static void write_batch(void *run, void *item)
+{
+	const fm_run_t *r = run;
+	fm_batch_t *b = item;
 	bb_str_t s = {0, 0, 0};
 	int i;
 	for (i = 0; i < b->n; ++i) {
@@ -95,27 +101,13 @@ static void write_batch(const fm_run_t *r, const fm_batch_t *b)
 		bb_putc(&s, '\n');
 		bb_putsn(&s, b->res.text + t0, (size_t)(t1 - t0));
 		bb_puts(&s, "//\n");
-		if (s.l >= (1 << 20)) {
-			if (fwrite(s.s, 1, s.l, stdout) != s.l) bb_fatal("main_fastmap", "fail to write the output");
-			s.l = 0;
-		}
+		bb_str_write(&s, 1 << 20, "main_fastmap");
 	}
-	if (s.l && fwrite(s.s, 1, s.l, stdout) != s.l) bb_fatal("main_fastmap", "fail to write the output");
-	free(s.s);
+	bb_str_write(&s, 0, "main_fastmap");
+	batch_free(b);   /* the device batch too: its pinned text buffer held the EM lines until now */
 }
 
-static void *writer_main(void *arg)
-{
-	fm_run_t *r = arg;
-	fm_batch_t *b;
-	while ((b = bb_mbox_get(&r->to_write)) != 0) {
-		double t0 = bb_realtime();
-		write_batch(r, b);
-		batch_free(b);   /* the device batch too: its pinned text buffer held the EM lines until now */
-		r->t_write += bb_realtime() - t0;
-	}
-	return 0;
-}
+static const bb_pipe_ops_t ops = { read_all, run_device, write_batch };
 
 static void usage(int min_len, int w, int min_intv, int max_len, uint64_t max_intv)
 {
@@ -135,11 +127,9 @@ int bb_fastmap_main(int argc, char *argv[])
 	int c, min_iwidth = 20, min_len = 17, print_seq = 0, min_intv = 1, max_len = 0x7fffffff;
 	uint64_t max_intv = 0;
 	bwaidx_t *idx;
-	bwag_ctx_t *ctx;
 	fm_run_t run;
-	bwag_fastmap_par_t par;
-	pthread_t th_r, th_w;
-	double t0, t_load, t_dev = 0;
+	bb_pipe_busy_t busy;
+	double t0, t_load;
 	const char *e;
 
 	while ((c = getopt(argc, argv, "w:l:pi:I:L:")) >= 0) {   /* fastmap.c:419-429 */
@@ -161,33 +151,14 @@ int bb_fastmap_main(int argc, char *argv[])
 	if ((run.fq = bb_fq_open(argv[optind + 1])) == 0) bb_fatal("main_fastmap", "fail to open file '%s'", argv[optind + 1]);
 	t0 = bb_realtime();
 	if ((idx = bb_idx_from_resident(argv[optind])) == 0 && (idx = bwa_idx_load(argv[optind], BWA_IDX_ALL)) == 0) { bb_fq_close(run.fq); return 1; }
-	ctx = bb_device_attach(idx->bwt, idx->bns, idx->pac);   /* fails here, before any output, if there is no GPU */
+	run.ctx = bb_device_attach(idx->bwt, idx->bns, idx->pac);   /* fails here, before any output, if there is no GPU */
 	t_load = bb_realtime() - t0;
-	memset(&par, 0, sizeof(par));
-	par.min_len = min_len; par.min_intv = min_intv; par.max_intv = max_intv; par.max_iwidth = min_iwidth;
-
-	bb_mbox_init(&run.to_dev); bb_mbox_init(&run.to_write);
-	pthread_create(&th_r, 0, reader_main, &run);
-	pthread_create(&th_w, 0, writer_main, &run);
-	for (;;) {
-		fm_batch_t *b = bb_mbox_get(&run.to_dev);
-		double t1 = bb_realtime();
-		int rc;
-		if (!b) break;
-		if ((b->dev = bwag_batch_begin(ctx, b->n, b->codes, b->off)) == 0) bb_fatal("main_fastmap", "cannot start a device batch: %s", bwag_last_error());
-		rc = bwag_fastmap(b->dev, &par, &b->res);
-		if (rc == BWAG_UNSUPPORTED) { fprintf(stderr, "[E::%s] this build has no device SMEM lister\n", "main_fastmap"); exit(1); }
-		if (rc != 0) bb_fatal("main_fastmap", "device SMEM listing failed: %s", bwag_last_error());
-		t_dev += bb_realtime() - t1;
-		bb_mbox_put(&run.to_write, b);
-	}
-	bb_mbox_put(&run.to_write, 0);
-	pthread_join(th_r, 0);
-	pthread_join(th_w, 0);
+	run.par.min_len = min_len; run.par.min_intv = min_intv; run.par.max_intv = max_intv; run.par.max_iwidth = min_iwidth;
+	bb_pipe_run(&ops, &run, &busy);
 	if (fflush(stdout) != 0 || ferror(stdout)) bb_fatal("main_fastmap", "fail to write the output");
 	if (getenv("BWA_B200_PROFILE"))
 		fprintf(stderr, "[prof] fastmap: index load %.3f s; busy time of the reader %.3f s, the device %.3f s, the writer %.3f s; total %.3f s\n",
-		        t_load, run.t_read, t_dev, run.t_write, bb_realtime() - t0);
+		        t_load, busy.read, busy.device, busy.write, bb_realtime() - t0);
 	bb_fq_close(run.fq);
 	bwa_idx_destroy(idx);
 	return 0;

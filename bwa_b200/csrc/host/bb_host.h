@@ -192,8 +192,21 @@ _Static_assert(offsetof(aln_opt_t, seed_len) == 48 && offsetof(aln_opt_t, n_thre
 bb_reads_t *bb_read_group(bb_fq_t *fq, int mode, int trim_qual, int n_max, int keep, int max_len, const char *who);
 void bb_reads_free(bb_reads_t *g);
 
-/* ---- `bwa-b200 samse` (bb_samse.c) ---- */
+/* ---- `bwa-b200 samse` (bb_samse.c), and the parts of bwase.c that `sampe` uses too ---- */
 int bb_samse_main(int argc, char *argv[]);
+/* bwase_initialize's g_log_n, and a private erand48 state seeded as srand48(bns->seed) seeds drand48: the same sequence, which
+ * nothing else in the process can disturb */
+typedef struct { unsigned short rng[3]; int log_n[256]; } bb_aln2seq_t;
+void bb_aln2seq_init(bb_aln2seq_t *s, const bntseq_t *bns);
+/* the hit bwa_aln2seq_core chooses from a read's .sai records (bwase.c:22-48): one draw per best-score interval, a second when it
+ * is taken.  sa, ref_shift, score and the differences are the last interval taken; they stay untouched when none is. */
+typedef struct { uint64_t sa; int ref_shift, score; uint32_t c1, c2; uint8_t type, n_mm, n_gapo, n_gape; } bb_hit_t;
+void bb_choose_hit(bb_aln2seq_t *s, int n_aln, const bwag_aln1_t *aln, bb_hit_t *h);
+/* bwa_approx_mapQ (bwase.c:101-110) of a read of len bases searched, with the max_diff of opt (samse: its .sai; sampe: .sai 2) */
+int bb_approx_mapq(const bb_aln2seq_t *s, const aln_opt_t *opt, int len, const bb_hit_t *h);
+void bb_upload_holes(bwag_ctx_t *ctx, const bntseq_t *bns, const char *who);   /* bwag_ctx_set_ambs; fatal on failure */
+/* one SAM record: read r's name + part A + QUAL (reversed under BWAG_REC_QREV, "*" without) + part B + "\n" */
+void bb_splice_sam(bb_str_t *s, const bb_reads_t *rd, int r, const bwag_samrec_t *rec, const char *text);
 
 /* ---- `bwa-b200 sampe` (bb_sampe.c) ---- */
 int bb_sampe_main(int argc, char *argv[]);

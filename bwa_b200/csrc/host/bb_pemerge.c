@@ -1,16 +1,15 @@
 /* bb_pemerge.c -- `bwa-b200 pemerge`: the merged and unmerged read pairs of the reference's `bwa pemerge` (pemerge.c:217-291) byte for
  * byte, with the alignment, the tests, the merge and the records on the GPU (bwag_pemerge, bwag_pemerge.cu).
  *
- * Three threads overlap, as in samse: a reader takes the pairs with bseq_read (two files, or one interleaved file; trim_readno, gzip,
- * "-" for stdin and the two "fewer sequences" warnings come with it), drops an odd last read as process_seqs does, and copies each
- * batch of BWA_B200_PEMERGE_CHUNK pairs into page-locked buffers: sequences, qualities and names, one copy per byte; the calling
- * thread runs a batch on the device; a writer prints the records the device wrote, in input order.  Pairs are independent and the
- * reference only breaks its batches at an even read count, so our batch size shows in no byte; the reader still calls bseq_read with
- * the reference's size, because a call that reads no base probes file 2 and so consumes one of its records.  The nine counts go to
- * stderr after the output.  BWA_B200_PROFILE=1 reports the busy time of the three threads. */
+ * It runs on the pipeline of bb_util.h: the reader takes the pairs with bseq_read (two files, or one interleaved file; trim_readno,
+ * gzip, "-" for stdin and the two "fewer sequences" warnings come with it), drops an odd last read as process_seqs does, and copies
+ * each batch of BWA_B200_PEMERGE_CHUNK pairs into page-locked buffers: sequences, qualities and names, one copy per byte; the writer
+ * prints the records the device wrote and returns the batch, buffers kept, to a free list for the reader.  Pairs are independent
+ * and the reference only breaks its batches at an even read count, so our batch size shows in no byte; the reader still calls
+ * bseq_read with the reference's size, because a call that reads no base probes file 2 and so consumes one of its records.  The
+ * nine counts go to stderr after the output.  BWA_B200_PROFILE=1 reports the busy time of the three threads. */
 #include <unistd.h>
 #include <errno.h>
-#include <pthread.h>
 #include "bb_host.h"
 
 #define PM_GROUP_BASES (1 << 26)   /* bases per group of pairs the reader gathers; no byte depends on it */
@@ -43,11 +42,11 @@ typedef struct {
 	bb_fq_t *fq[2];
 	int chunk;
 	int ref_chunk;                /* the reference's bseq_read size, n_threads * 10000000 as an int */
-	bb_mbox_t to_dev, to_write;
 	pthread_mutex_t mu; pm_batch_t *free_list;   /* batches the writer is done with, buffers kept */
-	int64_t cnt[9];
+	bwag_ctx_t *ctx;
+	bwag_pemerge_par_t par;
+	int64_t cnt[9];               /* writer */
 	int eof;
-	double t_read, t_write;
 	long long n_pairs;
 } pm_run_t;
 
@@ -135,47 +134,42 @@ static bseq1_t *read_group(pm_run_t *r, int *n_)
 	return n ? g : (free(g), (bseq1_t *)0);
 }
 
-static void *reader_main(void *arg)
+static void read_all(bb_pipe_t *p, void *run)
 {
-	pm_run_t *r = arg;
+	pm_run_t *r = run;
 	while (!r->eof) {
 		int n, i, beg;
-		double t0 = bb_realtime();
 		bseq1_t *seqs = read_group(r, &n);
-		r->t_read += bb_realtime() - t0;
 		if (!seqs) break;
 		const int np = n >> 1;
-		for (beg = 0; beg < np; beg += r->chunk) {
-			const int end = beg + r->chunk < np ? beg + r->chunk : np;
-			t0 = bb_realtime();
-			pm_batch_t *b = fill(r, seqs, beg, end);
-			r->t_read += bb_realtime() - t0;
-			bb_mbox_put(&r->to_dev, b);
-		}
-		t0 = bb_realtime();
+		for (beg = 0; beg < np; beg += r->chunk) bb_pipe_to_device(p, fill(r, seqs, beg, beg + r->chunk < np ? beg + r->chunk : np));
 		for (i = 0; i < n; ++i) { free(seqs[i].name); free(seqs[i].comment); free(seqs[i].seq); free(seqs[i].qual); }
 		free(seqs);
-		r->t_read += bb_realtime() - t0;
 	}
-	bb_mbox_put(&r->to_dev, 0);
-	return 0;
 }
 
-static void *writer_main(void *arg)
+static void run_device(bb_pipe_t *p, void *run, void *item)
 {
-	pm_run_t *r = arg;
-	pm_batch_t *b;
-	while ((b = bb_mbox_get(&r->to_write)) != 0) {
-		double t0 = bb_realtime();
-		int k;
-		if (b->res.n_text && fwrite(b->res.text, 1, (size_t)b->res.n_text, stdout) != (size_t)b->res.n_text) bb_fatal(WHO, "fail to write the output");
-		for (k = 0; k < 9; ++k) r->cnt[k] += b->res.cnt[k];
-		r->n_pairs += b->n;
-		batch_put(r, b);
-		r->t_write += bb_realtime() - t0;
-	}
-	return 0;
+	pm_run_t *r = run;
+	pm_batch_t *b = item;
+	if ((b->dev = bwag_batch_begin(r->ctx, 2 * b->n, b->seq.p, b->off.p)) == 0) bb_fatal(WHO, "cannot start a device batch: %s", bwag_last_error());
+	r->par.qual = b->qual.p; r->par.has_qual = b->hasq.p; r->par.names = b->names.p; r->par.name_off = b->noff.p;
+	if (bwag_pemerge(b->dev, &r->par, &b->res) != 0) bb_fatal(WHO, "device pemerge failed: %s", bwag_last_error());
+	bb_pipe_to_writer(p, b);
 }
+
+static void write_batch(void *run, void *item)
+{
+	pm_run_t *r = run;
+	pm_batch_t *b = item;
+	int k;
+	if (b->res.n_text && fwrite(b->res.text, 1, (size_t)b->res.n_text, stdout) != (size_t)b->res.n_text) bb_fatal(WHO, "fail to write the output");
+	for (k = 0; k < 9; ++k) r->cnt[k] += b->res.cnt[k];
+	r->n_pairs += b->n;
+	batch_put(r, b);
+}
+
+static const bb_pipe_ops_t ops = { read_all, run_device, write_batch };
 
 static bb_fq_t *open_reads(const char *fn)
 {
@@ -192,10 +186,9 @@ int bb_pemerge_main(int argc, char *argv[])
 {
 	int c, flag = 0, min_ovlp = 10, q_thres = 70, n_threads = 1, i;
 	pm_run_t run;
-	bwag_ctx_t *ctx;
-	bwag_pemerge_par_t par;
-	pthread_t th_r, th_w;
-	double t0 = bb_realtime(), t_dev = 0;
+	bwag_pemerge_par_t *par = &run.par;
+	bb_pipe_busy_t busy;
+	double t0 = bb_realtime();
 	const char *e;
 	while ((c = getopt(argc, argv, "muQ:t:T:")) >= 0) {   /* pemerge.c:227-234 */
 		if (c == 'm') flag |= 1;
@@ -227,19 +220,18 @@ int bb_pemerge_main(int argc, char *argv[])
 		}
 		run.fq[1] = open_reads(argv[optind + 1]);
 	}
-	if ((ctx = bwag_ctx_create_bare(-1)) == 0) bb_fatal(WHO, "cannot use the GPU: %s", bwag_last_error());   /* before any output */
-	memset(&par, 0, sizeof(par));
-	par.T = 5 * min_ovlp; par.q_thres = q_thres; par.q_def = 20; par.flag = flag;
-	par.merge = n_threads > 0;   /* -t 0: the reference starts no worker, so no pair is tried */
+	if ((run.ctx = bwag_ctx_create_bare(-1)) == 0) bb_fatal(WHO, "cannot use the GPU: %s", bwag_last_error());   /* before any output */
+	par->T = 5 * min_ovlp; par->q_thres = q_thres; par->q_def = 20; par->flag = flag;
+	par->merge = n_threads > 0;   /* -t 0: the reference starts no worker, so no pair is tried */
 	{   /* a batch of no pairs: does this build have the device stage at all? */
 		static const uint8_t none[1] = {0};
 		static const int64_t zero[1] = {0};
 		bwag_pemerge_t res;
-		bwag_batch_t *b = bwag_batch_begin(ctx, 0, none, zero);
+		bwag_batch_t *b = bwag_batch_begin(run.ctx, 0, none, zero);
 		int rc;
 		if (!b) bb_fatal(WHO, "cannot start a device batch: %s", bwag_last_error());
-		par.qual = none; par.has_qual = none; par.names = (const char *)none; par.name_off = zero;
-		rc = bwag_pemerge(b, &par, &res);
+		par->qual = none; par->has_qual = none; par->names = (const char *)none; par->name_off = zero;
+		rc = bwag_pemerge(b, par, &res);
 		bwag_batch_end(b);
 		if (rc == BWAG_UNSUPPORTED) { fprintf(stderr, "[E::%s] this build has no device pemerge\n", WHO); exit(1); }
 		if (rc != 0) bb_fatal(WHO, "device pemerge failed: %s", bwag_last_error());
@@ -247,30 +239,14 @@ int bb_pemerge_main(int argc, char *argv[])
 	run.ref_chunk = (int)((uint32_t)n_threads * 10000000u);   /* pemerge.c:52,272: wraps above -t 214 */
 	run.chunk = (e = getenv("BWA_B200_PEMERGE_CHUNK")) != 0 && atoi(e) > 0 ? atoi(e) : PM_CHUNK;
 	pthread_mutex_init(&run.mu, 0);
-	bb_mbox_init(&run.to_dev); bb_mbox_init(&run.to_write);
-	pthread_create(&th_r, 0, reader_main, &run);
-	pthread_create(&th_w, 0, writer_main, &run);
-	for (;;) {
-		pm_batch_t *b = bb_mbox_get(&run.to_dev);
-		double t1 = bb_realtime();
-		int rc;
-		if (!b) break;
-		if ((b->dev = bwag_batch_begin(ctx, 2 * b->n, b->seq.p, b->off.p)) == 0) bb_fatal(WHO, "cannot start a device batch: %s", bwag_last_error());
-		par.qual = b->qual.p; par.has_qual = b->hasq.p; par.names = b->names.p; par.name_off = b->noff.p;
-		if ((rc = bwag_pemerge(b->dev, &par, &b->res)) != 0) bb_fatal(WHO, "device pemerge failed: %s", bwag_last_error());
-		t_dev += bb_realtime() - t1;
-		bb_mbox_put(&run.to_write, b);
-	}
-	bb_mbox_put(&run.to_write, 0);
-	pthread_join(th_r, 0);
-	pthread_join(th_w, 0);
+	bb_pipe_run(&ops, &run, &busy);
 	if (fflush(stdout) != 0 || ferror(stdout)) bb_fatal(WHO, "fail to write the output");
 	for (i = 0; i <= 8; ++i) fprintf(stderr, "%12ld %s\n", (long)run.cnt[i], err_msg[i]);   /* pemerge.c:277-279 */
 	if (getenv("BWA_B200_PROFILE"))
 		fprintf(stderr, "[prof] pemerge: busy time of the reader %.3f s, the device %.3f s, the writer %.3f s; %lld pairs; total %.3f s\n",
-		        run.t_read, t_dev, run.t_write, run.n_pairs, bb_realtime() - t0);
+		        busy.read, busy.device, busy.write, run.n_pairs, bb_realtime() - t0);
 	while (run.free_list) { pm_batch_t *b = run.free_list; run.free_list = b->next; batch_destroy(b); }
 	bb_fq_close(run.fq[0]); bb_fq_close(run.fq[1]);
-	bwag_ctx_destroy(ctx);
+	bwag_ctx_destroy(run.ctx);
 	return 0;
 }

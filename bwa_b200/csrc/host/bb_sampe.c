@@ -2,10 +2,10 @@
  * .sai files of `bwa aln` or `bwa-b200 aln`, with the suffix-array lookups, the mate rescue's alignments, the gapped refinement,
  * MD/NM and the SAM text on the GPU (bwag_pe_sa2pos, bwag_localsw, bwag_pe_global, bwag_sampe; bwag_sampe.cu).
  *
- * Three threads overlap, as in samse: a reader parses the two read files (bb_read_group, file 1 with the mode and trimming of .sai
- * 1, file 2 with those of .sai 2) in the reference's groups of 262144 pairs, reads the two .sai files pair by pair and chooses each
- * read's hit and single-end mapping quality (bwa_aln2seq_core, bwa_approx_mapQ) with a private erand48 state seeded as the
- * reference's srand48(bns->seed); the calling thread runs a group on the device; a writer prints it.  Per group:
+ * It runs on the pipeline of bb_util.h: the reader parses the two read files (bb_read_group, file 1 with the mode and trimming of
+ * .sai 1, file 2 with those of .sai 2) in the reference's groups of 262144 pairs, reads the two .sai files pair by pair and chooses
+ * each read's hit and single-end mapping quality with samse's bwa_aln2seq_core and bwa_approx_mapQ (bb_samse.c); the device stage
+ * runs a group and cuts it into writer batches.  Per group:
  *   P1  the chosen hits' positions (bwag_pe_sa2pos), then the insert-size model (infer_isize, host libm, with last_ii and -A);
  *   P2  per batch of BWA_B200_SAMPE_CHUNK pairs, cut further by a budget of rows: every row of every interval the pairing or XA can
  *       need, resolved once, with bwa_sa2pos for both reference lengths; the pairing (pairing(), bwape.c:156-254) and the XA
@@ -17,12 +17,10 @@
  * BWA_B200_PROFILE=1 reports the index load, the busy time of the three threads and the work of each step. */
 #include <unistd.h>
 #include <math.h>
-#include <pthread.h>
 #include "bb_host.h"
 
 #define PE_GROUP    0x40000       /* pairs per bwa_read_seq call (bwape.c:675) */
 #define PE_MAX_LEN  (1 << 20)
-#define PE_AVG_ERR  0.02          /* BWA_AVG_ERR */
 #define PE_ROWS     ((int64_t)1 << 22)   /* rows resolved per device call (P2): 34 bytes each on the device */
 #define SW_MIN_MATCH_LEN 20
 #define SW_MIN_MAPQ 17
@@ -33,6 +31,7 @@
 #define WHO "bwa_sai2sam_pe_core"
 
 typedef struct { double avg, std, ap_prior; uint64_t low, high, high_bayesian; } isize_info_t;
+typedef struct { long long n_rows, n_sorted, n_local, n_global, n_refine; double t_pair, t_sw, t_dev_calls; } pe_work_t;
 
 typedef struct {                  /* one end as bwa_seq_t keeps it */
 	uint64_t sa, pos;
@@ -50,8 +49,6 @@ typedef struct {
 	pe_end_t *e;                  /* [2n]: pair i = e[2i], e[2i + 1] */
 	bwag_aln1_t *aln; int64_t n_aln, m_aln;
 	char *bc; int64_t *bc_off; int *l_bc;   /* each pair's barcode: both reads' barcodes concatenated (bwape.c:703-706) */
-	int eof;                      /* the .sai ended inside the group: nothing of it is printed */
-	char *err;                    /* the group cannot be printed: the command fails with this message once the earlier ones are out */
 	int last;                     /* file 2 ended inside this group: the reference prints nothing after it */
 } pe_group_t;
 
@@ -59,8 +56,6 @@ typedef struct {
 	pe_group_t *g; int beg, n, last_of_group;
 	bwag_batch_t *dev;
 	bwag_sam_t res;
-	char *err;                    /* the group cannot be printed: this message, once the earlier groups are out */
-	int sai_eof;                  /* a .sai file ended inside the group */
 } pe_batch_t;
 
 typedef struct {
@@ -69,19 +64,23 @@ typedef struct {
 	aln_opt_t opt[2];
 	int max_isize, max_occ, n_multi, N_multi, is_sw, force_isize, chunk;
 	double ap_prior;
-	unsigned short rng[3];
-	int log_n[256];
-	bb_mbox_t to_dev, to_write;
-	int stop;                     /* writer: an error group, the end of a .sai file or mismatched names was met */
+	bb_aln2seq_t se;
+	/* reader: a .sai file ended inside a group, or a group cannot be printed (the message); the reader stops there and the command
+	 * fails once the earlier groups are out */
 	int sai_eof; char *err;
-	double t_read, t_write;
+	char *bad_names;              /* writer: the message of the first pair with different names; nothing is printed after it */
+	int no_device;                /* device stage: this build has no device sampe; the groups the reader still hands on are dropped */
+	bwag_ctx_t *ctx;
+	const bwaidx_t *idx;
+	isize_info_t last_ii;
+	pe_work_t work;
 } pe_run_t;
 
 static void group_free(pe_group_t *g)
 {
 	if (!g) return;
 	bb_reads_free(g->rd[0]); bb_reads_free(g->rd[1]);
-	free(g->e); free(g->aln); free(g->bc); free(g->bc_off); free(g->l_bc); free(g->err);
+	free(g->e); free(g->aln); free(g->bc); free(g->bc_off); free(g->l_bc);
 	free(g);
 }
 
@@ -93,45 +92,7 @@ static char *xstrdup_printf(const char *fmt, const char *a, const char *b)
 	return s;
 }
 
-/* bwa_aln2seq_core(n_aln, aln, p, 1, 0) (bwase.c:22-48): the reference's integer widths, 28-bit c1/c2 */
-static void choose_hit(pe_run_t *r, int n_aln, const bwag_aln1_t *aln, pe_end_t *p)
-{
-	int i, cnt, best;
-	if (n_aln == 0) { p->type = 0; p->c1 = p->c2 = 0; return; }
-	best = (int)(aln[0].bits >> 24 & 0xfffff);
-	for (i = cnt = 0; i < n_aln; ++i) {
-		const bwag_aln1_t *q = aln + i;
-		const uint64_t w = q->l - q->k + 1;
-		if ((int)(q->bits >> 24 & 0xfffff) > best) break;
-		if (erand48(r->rng) * (double)(w + (uint64_t)(int64_t)cnt) > (double)cnt) {
-			p->n_mm = (uint8_t)(q->bits & 0xff); p->n_gapo = (uint8_t)(q->bits >> 8 & 0xff); p->n_gape = (uint8_t)(q->bits >> 16 & 0xff);
-			p->ref_shift = (int)(q->bits >> 54 & 0x3ff) - (int)(q->bits >> 44 & 0x3ff);
-			p->score = (int)(q->bits >> 24 & 0xfffff);
-			p->sa = q->k + (uint64_t)((double)w * erand48(r->rng));
-		}
-		cnt = (int)((uint64_t)(int64_t)cnt + w);
-	}
-	p->c1 = (uint32_t)((uint64_t)(int64_t)cnt & 0xfffffff);
-	for (; i < n_aln; ++i) cnt = (int)((uint64_t)(int64_t)cnt + (aln[i].l - aln[i].k + 1));
-	p->c2 = (uint32_t)(((uint64_t)(int64_t)cnt - p->c1) & 0xfffffff);
-	p->type = p->c1 > 1 ? 2 : 1;
-}
-
-/* bwa_approx_mapQ (bwase.c:101-110) with the max_diff of bwape.c:296 */
-static int approx_mapq(const pe_run_t *r, const pe_end_t *p)
-{
-	const aln_opt_t *o = &r->opt[1];
-	const int mm = o->fnr > 0.0 ? bb_cal_maxdiff(p->len, PE_AVG_ERR, o->fnr) : o->max_diff;
-	int n;
-	if (p->c1 == 0) return 23;
-	if (p->c1 > 1) return 0;
-	if (p->n_mm == mm) return 25;
-	if (p->c2 == 0) return 37;
-	n = p->c2 >= 255 ? 255 : (int)p->c2;
-	return 23 < r->log_n[n] ? 0 : 23 - r->log_n[n];
-}
-
-/* the next group with its hits chosen; NULL at the end of file 1 */
+/* the next group with its hits chosen; NULL at the end of file 1.  r->sai_eof or r->err: the group cannot be printed */
 static pe_group_t *read_group(pe_run_t *r)
 {
 	bb_reads_t *rd0 = bb_read_group(r->fq[0], r->opt[0].mode, r->opt[0].trim_qual, PE_GROUP, 1, PE_MAX_LEN, WHO), *rd1;
@@ -145,7 +106,7 @@ static pe_group_t *read_group(pe_run_t *r)
 	if (g->n > rd0->n) {       /* the reference reads past its array of file-1 reads here */
 		char a[32];
 		snprintf(a, sizeof(a), "%d", rd0->n);
-		g->err = xstrdup_printf("the first read file has fewer reads than the second (%s pairs in its last group)%s", a, 0);
+		r->err = xstrdup_printf("the first read file has fewer reads than the second (%s pairs in its last group)%s", a, 0);
 		return g;
 	}
 	if (g->n < rd0->n) g->last = 1;
@@ -157,7 +118,7 @@ static pe_group_t *read_group(pe_run_t *r)
 			const char *b0 = rd0->bc[i] >= 0 ? rd0->text.s + rd0->bc[i] : "", *b1 = rd1->bc[i] >= 0 ? rd1->text.s + rd1->bc[i] : "";
 			const int l = (int)(strlen(b0) + strlen(b1));
 			if (l > BB_MAX_BCLEN) {
-				g->err = xstrdup_printf("pair '%s': its two barcodes together are longer than 63 bases%s", rd0->text.s + rd0->name[i], 0);
+				r->err = xstrdup_printf("pair '%s': its two barcodes together are longer than 63 bases%s", rd0->text.s + rd0->name[i], 0);
 				free(bc.s);
 				return g;
 			}
@@ -170,37 +131,36 @@ static pe_group_t *read_group(pe_run_t *r)
 		int j;
 		for (j = 0; j < 2; ++j) {
 			pe_end_t *p = &g->e[2 * i + j];
+			bb_hit_t h = {0};
 			int32_t n_aln;
-			if (fread(&n_aln, 4, 1, r->fp_sa[j]) != 1 || n_aln < 0) { g->eof = 1; return g; }
+			if (fread(&n_aln, 4, 1, r->fp_sa[j]) != 1 || n_aln < 0) { r->sai_eof = 1; return g; }
 			if (g->n_aln + n_aln > g->m_aln) {
 				while (g->n_aln + n_aln > g->m_aln) g->m_aln = g->m_aln ? g->m_aln << 1 : 4096;
 				g->aln = bb_realloc(g->aln, sizeof(*g->aln) * (size_t)g->m_aln);
 			}
-			if (n_aln > 0 && fread(g->aln + g->n_aln, sizeof(*g->aln), (size_t)n_aln, r->fp_sa[j]) != (size_t)n_aln) { g->eof = 1; return g; }
+			if (n_aln > 0 && fread(g->aln + g->n_aln, sizeof(*g->aln), (size_t)n_aln, r->fp_sa[j]) != (size_t)n_aln) { r->sai_eof = 1; return g; }
 			p->aln_beg = g->n_aln; p->n_aln = n_aln; g->n_aln += n_aln;
 			p->len = g->rd[j]->len[i];
 			p->flag = F_PD | (j == 0 ? F_R1 : F_R2);
-			choose_hit(r, n_aln, g->aln + p->aln_beg, p);
-			if (p->type) p->seq_q = p->mapq = (uint8_t)approx_mapq(r, p);
+			bb_choose_hit(&r->se, n_aln, g->aln + p->aln_beg, &h);
+			p->sa = h.sa; p->ref_shift = h.ref_shift; p->score = h.score; p->c1 = h.c1; p->c2 = h.c2;
+			p->type = h.type; p->n_mm = h.n_mm; p->n_gapo = h.n_gapo; p->n_gape = h.n_gape;
+			if (p->type) p->seq_q = p->mapq = (uint8_t)bb_approx_mapq(&r->se, &r->opt[1], p->len, &h);
 		}
 	}
 	return g;
 }
 
-static void *reader_main(void *arg)
+static void read_all(bb_pipe_t *p, void *run)
 {
-	pe_run_t *r = arg;
-	for (;;) {
-		double t0 = bb_realtime();
-		pe_group_t *g = read_group(r);
-		r->t_read += bb_realtime() - t0;
-		if (!g) break;
-		const int stop = g->eof || g->err || g->last;   /* read before the hand-over: the other threads may free g at once */
-		bb_mbox_put(&r->to_dev, g);
-		if (stop) break;
+	pe_run_t *r = run;
+	pe_group_t *g;
+	while ((g = read_group(r)) != 0) {
+		if (r->sai_eof || r->err) { group_free(g); return; }   /* nothing of this group is printed */
+		const int last = g->last;   /* read before the hand-over: the other threads may free g at once */
+		bb_pipe_to_device(p, g);
+		if (last) return;
 	}
-	bb_mbox_put(&r->to_dev, 0);
-	return 0;
 }
 
 /* ---------------------------------------------------------------- insert size (infer_isize, bwape.c:81-154) */
@@ -374,7 +334,7 @@ static int pairing(const pe_run_t *r, pe_end_t *p[2], const int full_len[2], con
 			else if ((s.subo_score >> 32) - (s.o_score >> 32) > (uint64_t)(int64_t)(r->opt[1].s_mm * 10)) mapq_p = 23;
 			else {
 				const int n = s.subo_n > 255 ? 255 : s.subo_n;
-				mapq_p = (int)(((s.subo_score >> 32) - (s.o_score >> 32)) / 2 - (uint64_t)(int64_t)r->log_n[n]);
+				mapq_p = (int)(((s.subo_score >> 32) - (s.o_score >> 32)) / 2 - (uint64_t)(int64_t)r->se.log_n[n]);
 				if (mapq_p < 0) mapq_p = 0;
 			}
 		}
@@ -412,7 +372,6 @@ typedef struct {                  /* what a batch builds for bwag_sampe */
 	uint32_t *cig; int64_t n_cig, m_cig;
 } pe_lists_t;
 
-typedef struct { long long n_rows, n_sorted, n_local, n_global, n_refine; double t_pair, t_sw, t_dev_calls; } pe_work_t;
 
 static void push_multi(pe_lists_t *L, const bwag_aln1_t *q, int64_t pos, int strand)
 {
@@ -800,7 +759,7 @@ static pe_batch_t *run_batch(pe_run_t *r, bwag_ctx_t *ctx, const bwaidx_t *idx, 
 			par.bc = g->bc ? g->bc + b0 : 0; par.l_bc = b1 - b0;
 		}
 		const int rc = bwag_sampe(bt->dev, &par, &bt->res, &past_end, &ng);
-		if (rc == BWAG_UNSUPPORTED) {   /* the caller stops the other threads and fails */
+		if (rc == BWAG_UNSUPPORTED) {   /* the caller drops the rest of the input and fails */
 			bwag_batch_end(bt->dev);
 			free(rd); free(pe); free(pos); free(str); free(L.multi); free(L.mpos); free(L.mstrand); free(L.cig); free(off); free(codes); free(bt);
 			return 0;
@@ -854,77 +813,64 @@ static void group_model(pe_run_t *r, bwag_ctx_t *ctx, const bwaidx_t *idx, pe_gr
 	*last_ii = *ii;
 }
 
-/* per read: name + part A + QUAL + part B + "\n"; after each pair the names are compared (bwape.c:709) */
-static int write_batch(pe_run_t *r, const pe_batch_t *b)
+static void run_device(bb_pipe_t *p, void *run, void *item)
 {
+	pe_run_t *r = run;
+	pe_group_t *g = item;
+	const int n = g->n;
+	isize_info_t ii;
+	if (r->no_device) { group_free(g); return; }
+	group_model(r, r->ctx, r->idx, g, &ii, &r->last_ii, &r->work);
+	if (n == 0) { group_free(g); return; }
+	/* the writer frees g with the group's last batch: nothing of g is touched once that batch is handed over */
+	for (int beg = 0; beg < n; beg += r->chunk) {
+		const int end = beg + r->chunk < n ? beg + r->chunk : n;
+		pe_batch_t *b = run_batch(r, r->ctx, r->idx, g, beg, end, &ii, &r->work);
+		if (!b) {
+			r->no_device = 1;
+			if (beg == 0) group_free(g);   /* no batch of g went out */
+			return;
+		}
+		b->last_of_group = end == n;
+		bb_pipe_to_writer(p, b);
+	}
+}
+
+/* per read: name + part A + QUAL + part B + "\n"; after each pair the names are compared (bwape.c:709).  Nothing is printed after
+ * a mismatch: the command fails with the reference's message once the other threads have stopped. */
+static void write_batch(void *run, void *item)
+{
+	pe_run_t *r = run;
+	pe_batch_t *b = item;
 	const pe_group_t *g = b->g;
 	bb_str_t s = {0, 0, 0};
 	int i, j, bad = -1;
-	for (i = 0; i < b->n && bad < 0; ++i) {
+	for (i = 0; i < b->n && bad < 0 && !r->bad_names; ++i) {
 		const int gi = b->beg + i;
-		for (j = 0; j < 2; ++j) {
-			const bb_reads_t *rd = g->rd[j];
-			const bwag_samrec_t *rec = &b->res.rec[2 * i + j];
-			const char *t = b->res.text + rec->off;
-			bb_puts(&s, rd->text.s + rd->name[gi]);
-			bb_putsn(&s, t, (size_t)rec->len_a);
-			if (rd->qual[gi] >= 0) {
-				const int full_len = (int)(rd->off[gi + 1] - rd->off[gi]);
-				bb_str_need(&s, (size_t)full_len);
-				bb_copy_text(s.s + s.l, rd->text.s + rd->qual[gi], full_len, (rec->flags & BWAG_REC_QREV) != 0);
-				s.l += full_len; s.s[s.l] = 0;
-			} else bb_putc(&s, '*');
-			bb_putsn(&s, t + rec->len_a, (size_t)rec->len_b);
-			bb_putc(&s, '\n');
-		}
+		for (j = 0; j < 2; ++j) bb_splice_sam(&s, g->rd[j], gi, &b->res.rec[2 * i + j], b->res.text);
 		if (strcmp(g->rd[0]->text.s + g->rd[0]->name[gi], g->rd[1]->text.s + g->rd[1]->name[gi]) != 0) bad = gi;
-		if (s.l >= (1 << 20)) {
-			if (fwrite(s.s, 1, s.l, stdout) != s.l) bb_fatal(WHO, "fail to write the output");
-			s.l = 0;
-		}
+		bb_str_write(&s, 1 << 20, WHO);
 	}
-	if (s.l && fwrite(s.s, 1, s.l, stdout) != s.l) bb_fatal(WHO, "fail to write the output");
-	free(s.s);
-	if (bad >= 0) {   /* the pair is out; the main thread fails with the reference's message once the others have stopped */
-		char *m = xstrdup_printf("paired reads have different names: \"%s\", \"%s\"\n", g->rd[0]->text.s + g->rd[0]->name[bad], g->rd[1]->text.s + g->rd[1]->name[bad]);
-		if (!r->err) r->err = m; else free(m);
-		return -1;
-	}
-	return 0;
+	bb_str_write(&s, 0, WHO);
+	if (bad >= 0)
+		r->bad_names = xstrdup_printf("paired reads have different names: \"%s\", \"%s\"\n", g->rd[0]->text.s + g->rd[0]->name[bad], g->rd[1]->text.s + g->rd[1]->name[bad]);
+	bwag_batch_end(b->dev);
+	if (b->last_of_group) group_free(b->g);
+	free(b);
 }
 
-static void *writer_main(void *arg)
-{
-	pe_run_t *r = arg;
-	pe_batch_t *b;
-	while ((b = bb_mbox_get(&r->to_write)) != 0) {
-		double t0 = bb_realtime();
-		if (b->sai_eof || b->err) {
-			if (!r->stop) { r->stop = 1; r->sai_eof = b->sai_eof; r->err = b->err; b->err = 0; }
-		} else if (!r->stop && write_batch(r, b) != 0) r->stop = 1;
-		if (b->dev) bwag_batch_end(b->dev);
-		if (b->last_of_group) group_free(b->g);
-		free(b->err); free(b);
-		r->t_write += bb_realtime() - t0;
-	}
-	return 0;
-}
+static const bb_pipe_ops_t ops = { read_all, run_device, write_batch };
 
 int bb_sampe_main(int argc, char *argv[])
 {
 	int c, i;
 	char *rg_line = 0, magic[2][4];
 	bwaidx_t *idx;
-	bwag_ctx_t *ctx;
 	pe_run_t run;
-	pthread_t th_r, th_w;
-	double t0, t_load, t_dev = 0;
-	pe_work_t work;
-	isize_info_t last_ii;
-	int no_device = 0;
+	bb_pipe_busy_t busy;
+	double t0, t_load;
 	const char *e;
 	memset(&run, 0, sizeof(run));
-	memset(&work, 0, sizeof(work));
 	run.max_isize = 500; run.max_occ = 100000; run.n_multi = 3; run.N_multi = 10; run.is_sw = 1; run.ap_prior = 1e-5;   /* bwa_init_pe_opt */
 	while ((c = getopt(argc, argv, "a:o:sPn:N:c:f:Ar:")) >= 0) {   /* bwape.c:740-756 */
 		switch (c) {
@@ -952,21 +898,11 @@ int bb_sampe_main(int argc, char *argv[])
 		free(rg_line);
 		return 1;
 	}
-	ctx = bb_device_attach(idx->bwt, idx->bns, idx->pac);   /* fails here, before any output, if there is no GPU */
-	{
-		const bntseq_t *bns = idx->bns;
-		int64_t *ao = bb_malloc(8 * (size_t)(bns->n_holes + 1));
-		int32_t *al = bb_malloc(4 * (size_t)(bns->n_holes + 1));
-		for (i = 0; i < bns->n_holes; ++i) ao[i] = bns->ambs[i].offset, al[i] = bns->ambs[i].len;
-		if (bwag_ctx_set_ambs(ctx, bns->n_holes, ao, al) != 0) bb_fatal(WHO, "cannot place the reference's holes on the GPU: %s", bwag_last_error());
-		free(ao); free(al);
-	}
+	run.idx = idx;
+	run.ctx = bb_device_attach(idx->bwt, idx->bns, idx->pac);   /* fails here, before any output, if there is no GPU */
+	bb_upload_holes(run.ctx, idx->bns, WHO);
 	t_load = bb_realtime() - t0;
-	{   /* srand48(bns->seed) */
-		const uint32_t seed = idx->bns->seed;
-		run.rng[0] = 0x330e; run.rng[1] = (unsigned short)(seed & 0xffff); run.rng[2] = (unsigned short)(seed >> 16);
-	}
-	for (i = 1; i != 256; ++i) run.log_n[i] = (int)(4.343 * log(i) + 0.5);
+	bb_aln2seq_init(&run.se, idx->bns);
 	for (i = 0; i < 2; ++i)
 		if ((run.fp_sa[i] = fopen(argv[optind + 1 + i], "r")) == 0) bb_fatal("xopen", "fail to open file '%s'", argv[optind + 1 + i]);
 	for (i = 0; i < 2; ++i) if (fread(magic[i], 1, 4, run.fp_sa[i]) != 4) bb_fatal("fread", "Unexpected end of file");
@@ -981,58 +917,16 @@ int bb_sampe_main(int argc, char *argv[])
 	}
 	bwa_print_sam_hdr(idx->bns, rg_line);
 	run.chunk = (e = getenv("BWA_B200_SAMPE_CHUNK")) != 0 && atoi(e) > 0 ? atoi(e) : PE_GROUP;   /* pairs per device batch */
-	last_ii.avg = -1.0; last_ii.std = -1.0; last_ii.ap_prior = 0; last_ii.low = last_ii.high = last_ii.high_bayesian = 0;
-
-	bb_mbox_init(&run.to_dev); bb_mbox_init(&run.to_write);
-	pthread_create(&th_r, 0, reader_main, &run);
-	pthread_create(&th_w, 0, writer_main, &run);
-	for (;;) {
-		pe_group_t *g = bb_mbox_get(&run.to_dev);
-		double t1 = bb_realtime();
-		isize_info_t ii;
-		if (!g) break;
-		/* the writer frees g with the group's last batch: nothing of g is touched once that batch is handed over */
-		if (g->eof || g->err) {   /* nothing of this group is printed; the command fails once the earlier ones are out */
-			pe_batch_t *b = bb_calloc(1, sizeof(*b));
-			b->g = g; b->last_of_group = 1;
-			b->sai_eof = g->eof; b->err = g->err; g->err = 0;
-			t_dev += bb_realtime() - t1;
-			bb_mbox_put(&run.to_write, b);
-			continue;
-		}
-		group_model(&run, ctx, idx, g, &ii, &last_ii, &work);
-		const int n = g->n;
-		if (n == 0) {
-			pe_batch_t *b = bb_calloc(1, sizeof(*b));
-			b->g = g; b->last_of_group = 1;
-			bb_mbox_put(&run.to_write, b);
-		}
-		for (int beg = 0; beg < n; beg += run.chunk) {
-			const int end = beg + run.chunk < n ? beg + run.chunk : n;
-			pe_batch_t *b = run_batch(&run, ctx, idx, g, beg, end, &ii, &work);
-			if (!b) { no_device = beg == 0 ? 1 : 2; break; }   /* 1: no batch of g went out */
-			b->last_of_group = end == n;
-			t_dev += bb_realtime() - t1;
-			bb_mbox_put(&run.to_write, b);
-			t1 = bb_realtime();
-		}
-		t_dev += bb_realtime() - t1;
-		if (no_device) {   /* let the reader finish, then stop the writer; the group is freed here, no batch of it went out */
-			pe_group_t *x;
-			if (no_device == 1) group_free(g);
-			while ((x = bb_mbox_get(&run.to_dev)) != 0) group_free(x);
-			break;
-		}
-	}
-	bb_mbox_put(&run.to_write, 0);
-	pthread_join(th_r, 0);
-	pthread_join(th_w, 0);
+	run.last_ii.avg = -1.0; run.last_ii.std = -1.0;
+	bb_pipe_run(&ops, &run, &busy);
 	if (fflush(stdout) != 0 || ferror(stdout)) bb_fatal(WHO, "fail to write the output");
 	if (getenv("BWA_B200_PROFILE"))
 		fprintf(stderr, "[prof] sampe: index load %.3f s; busy time of the reader %.3f s, the device %.3f s, the writer %.3f s; %lld rows sent to bwt_sa; %lld pairing candidates sorted; "
 		        "%lld mate local alignments, %lld mate global alignments; %lld gapped refinements; host part of the device thread: pairing and XA %.3f s, mate-rescue decisions %.3f s; total %.3f s\n",
-		        t_load, run.t_read, t_dev, run.t_write, work.n_rows, work.n_sorted, work.n_local, work.n_global, work.n_refine, work.t_pair, work.t_sw, bb_realtime() - t0);
-	if (no_device) { fprintf(stderr, "[E::%s] this build has no device sampe\n", WHO); exit(1); }
+		        t_load, busy.read, busy.device, busy.write, run.work.n_rows, run.work.n_sorted, run.work.n_local, run.work.n_global, run.work.n_refine,
+		        run.work.t_pair, run.work.t_sw, bb_realtime() - t0);
+	if (run.no_device) { fprintf(stderr, "[E::%s] this build has no device sampe\n", WHO); exit(1); }
+	if (run.bad_names) { fprintf(stderr, "[%s] %s\n", WHO, run.bad_names); exit(1); }   /* it comes before any group the reader refused */
 	if (run.sai_eof) { fprintf(stderr, "[fread] Unexpected end of file\n"); exit(1); }   /* err_fread_noeof, the earlier groups printed */
 	if (run.err) { fprintf(stderr, "[%s] %s\n", WHO, run.err); exit(1); }
 	for (i = 0; i < 2; ++i) { bb_fq_close(run.fq[i]); fclose(run.fp_sa[i]); }

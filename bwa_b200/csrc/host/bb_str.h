@@ -21,6 +21,16 @@ static inline void bb_str_need(bb_str_t *s, size_t extra)
 static inline void bb_putc(bb_str_t *s, int c) { bb_str_need(s, 1); s->s[s->l++] = (char)c; s->s[s->l] = 0; }
 static inline void bb_putsn(bb_str_t *s, const char *p, size_t n) { bb_str_need(s, n); memcpy(s->s + s->l, p, n); s->l += n; s->s[s->l] = 0; }
 static inline void bb_puts(bb_str_t *s, const char *p) { bb_putsn(s, p, strlen(p)); }
+/* a writer's output: once s holds at_least bytes, write them to stdout and empty s; at_least 0 writes the rest and frees s.  A short
+ * write is fatal (`who` names the command). */
+static inline void bb_str_write(bb_str_t *s, size_t at_least, const char *who)
+{
+	if (s->l && s->l >= at_least) {
+		if (fwrite(s->s, 1, s->l, stdout) != s->l) bb_fatal(who, "fail to write the output");
+		s->l = 0;
+	}
+	if (at_least == 0) { free(s->s); s->s = 0; s->m = 0; }
+}
 /* decimal text of a signed 64-bit value; identical digits to kputw/kputl (kstring.h:63-112) */
 static inline void bb_putl(bb_str_t *s, int64_t v)
 {

@@ -220,12 +220,13 @@ void bb_parallel_for_lane(int lane, int nt, void (*fn)(void *, long, int), void 
 	pthread_mutex_unlock(&g_pool.mu);
 }
 
-void bb_mbox_init(bb_mbox_t *m) { pthread_mutex_init(&m->mu, 0); pthread_cond_init(&m->cv, 0); m->slot = 0; m->full = 0; }
+void bb_mbox_init(bb_mbox_t *m) { pthread_mutex_init(&m->mu, 0); pthread_cond_init(&m->cv, 0); m->slot = 0; m->closed = 0; }
 void bb_mbox_put(bb_mbox_t *m, void *item)
 {
 	pthread_mutex_lock(&m->mu);
-	while (m->full) pthread_cond_wait(&m->cv, &m->mu);
-	m->slot = item; m->full = 1;
+	while (m->slot) pthread_cond_wait(&m->cv, &m->mu);
+	m->slot = item;
+	if (!item) m->closed = 1;
 	pthread_cond_broadcast(&m->cv);
 	pthread_mutex_unlock(&m->mu);
 }
@@ -233,11 +234,75 @@ void *bb_mbox_get(bb_mbox_t *m)
 {
 	void *item;
 	pthread_mutex_lock(&m->mu);
-	while (!m->full) pthread_cond_wait(&m->cv, &m->mu);
-	item = m->slot; m->slot = 0; m->full = 0;
+	while (!m->slot && !m->closed) pthread_cond_wait(&m->cv, &m->mu);
+	item = m->slot; m->slot = 0;
 	pthread_cond_broadcast(&m->cv);
 	pthread_mutex_unlock(&m->mu);
 	return item;
+}
+
+struct bb_pipe {
+	const bb_pipe_ops_t *ops;
+	void *run;
+	bb_mbox_t to_dev, to_write;
+	double wait_read, wait_dev;   /* time the reader and the device stage spent blocked in a hand-off */
+	bb_pipe_busy_t busy;
+};
+
+static void pipe_put(bb_mbox_t *m, void *item, double *wait)
+{
+	const double t0 = bb_realtime();
+	bb_mbox_put(m, item);
+	*wait += bb_realtime() - t0;
+}
+static void *pipe_get(bb_mbox_t *m, double *wait)
+{
+	const double t0 = bb_realtime();
+	void *item = bb_mbox_get(m);
+	*wait += bb_realtime() - t0;
+	return item;
+}
+void bb_pipe_to_device(bb_pipe_t *p, void *item) { pipe_put(&p->to_dev, item, &p->wait_read); }
+void bb_pipe_to_writer(bb_pipe_t *p, void *item) { pipe_put(&p->to_write, item, &p->wait_dev); }
+
+static void *pipe_reader(void *arg)
+{
+	bb_pipe_t *p = arg;
+	const double t0 = bb_realtime();
+	p->ops->read(p, p->run);
+	p->busy.read = bb_realtime() - t0 - p->wait_read;
+	bb_mbox_put(&p->to_dev, 0);
+	return 0;
+}
+
+static void *pipe_writer(void *arg)
+{
+	bb_pipe_t *p = arg;
+	const double t0 = bb_realtime();
+	double wait = 0;
+	void *item;
+	while ((item = pipe_get(&p->to_write, &wait)) != 0) p->ops->write(p->run, item);
+	p->busy.write = bb_realtime() - t0 - wait;
+	return 0;
+}
+
+void bb_pipe_run(const bb_pipe_ops_t *ops, void *run, bb_pipe_busy_t *busy)
+{
+	bb_pipe_t p;
+	pthread_t th_r, th_w;
+	double t0;
+	void *item;
+	memset(&p, 0, sizeof(p));
+	p.ops = ops; p.run = run;
+	bb_mbox_init(&p.to_dev); bb_mbox_init(&p.to_write);
+	if (pthread_create(&th_r, 0, pipe_reader, &p) != 0 || pthread_create(&th_w, 0, pipe_writer, &p) != 0) bb_fatal("bb_pipe_run", "pthread_create failed");
+	t0 = bb_realtime();
+	while ((item = pipe_get(&p.to_dev, &p.wait_dev)) != 0) ops->device(&p, run, item);
+	p.busy.device = bb_realtime() - t0 - p.wait_dev;
+	bb_mbox_put(&p.to_write, 0);
+	pthread_join(th_r, 0);
+	pthread_join(th_w, 0);
+	*busy = p.busy;
 }
 
 /* bwa_cal_maxdiff (bwtaln.c:42-54): the smallest k with P(more than k errors in l bases) < thres for Poisson(l*err) errors, in the

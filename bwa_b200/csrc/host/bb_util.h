@@ -49,13 +49,31 @@ int bb_parallel_ids(void);
 void bb_parallel_name(void (*fn)(void *, long, int), const char *name);   /* label a loop body for BWA_B200_PROFILE */
 void bb_parallel_report(void);   /* upper bound (exclusive) of the thread ids passed to loop bodies */
 
-/* single-slot mailbox between two threads: put waits while the slot is full, get while it is empty; the item NULL is a valid
- * message (the commands use it for the end of the input).  Stages connected by such mailboxes keep their order and at most one
- * item waits between two of them. */
-typedef struct { pthread_mutex_t mu; pthread_cond_t cv; void *slot; int full; } bb_mbox_t;
+/* single-slot mailbox: put waits while the slot is full, get while it is empty.  Putting NULL closes the box: once the item before
+ * it is taken, every get returns NULL, so any number of consumers see the end.  Stages connected by such mailboxes keep their order
+ * and at most one item waits between two of them. */
+typedef struct { pthread_mutex_t mu; pthread_cond_t cv; void *slot; int closed; } bb_mbox_t;
 void bb_mbox_init(bb_mbox_t *m);
 void bb_mbox_put(bb_mbox_t *m, void *item);
 void *bb_mbox_get(bb_mbox_t *m);
+
+/* The pipeline of fastmap, aln, samse, sampe and pemerge: three threads overlap.  A reader thread parses the input and hands items
+ * to the device stage; the device stage runs on the calling thread and hands its results to a writer thread, which prints and
+ * frees them.  Single-slot mailboxes join the stages, so output order is input order and at most one item waits between two
+ * stages.  A stage may hand on any number of items per call: aln, samse and pemerge cut a reader group into several device
+ * batches, sampe cuts a device group into several writer batches.  Items are never NULL.  bb_pipe_run returns once the reader
+ * has returned and every item is written; a stage that wants to stop early returns (reader) or drops what it gets (device).
+ * The busy time of a stage is its thread's wall time less the time it spent blocked in a hand-off (BWA_B200_PROFILE). */
+typedef struct bb_pipe bb_pipe_t;
+typedef struct {
+	void (*read)(bb_pipe_t *p, void *run);               /* reader thread: bb_pipe_to_device() per batch; returns at the end of the input */
+	void (*device)(bb_pipe_t *p, void *run, void *item);  /* calling thread: zero or more bb_pipe_to_writer() per item */
+	void (*write)(void *run, void *item);                 /* writer thread: prints the item and frees it */
+} bb_pipe_ops_t;
+typedef struct { double read, device, write; } bb_pipe_busy_t;
+void bb_pipe_run(const bb_pipe_ops_t *ops, void *run, bb_pipe_busy_t *busy);
+void bb_pipe_to_device(bb_pipe_t *p, void *item);
+void bb_pipe_to_writer(bb_pipe_t *p, void *item);
 
 /* bwa_cal_maxdiff (bwtaln.c:42-54): the most differences `bwa aln` allows in a read of l bases (-n as a fraction) */
 int bb_cal_maxdiff(int l, double err, double thres);
