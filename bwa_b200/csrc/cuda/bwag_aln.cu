@@ -17,6 +17,7 @@
  * A2 k_aln_gather: the hits in read order, at the offsets of a one-block scan of the counts (k_fm_scan32). */
 #include "bwag_dev.cuh"
 #include "bwag_kernels.h"
+#include "bwag_drv.h"
 
 #define A_M 0   /* states of a queue entry (bwtgap.c:11-13) */
 #define A_I 1
@@ -320,4 +321,116 @@ __global__ void k_aln_gather(int n_reads, const int *n_aln, const i64 *hit_beg, 
 		bwag_aln1_t *dst = out + off[r];
 		for (int j = 0; j < n; ++j) dst[j] = src[j];
 	}
+}
+
+/* ------------------------------------------------------------------------------------------------ host driver */
+
+#ifdef BWAG_CUSIM
+#define ALN_BUDGET ((i64)256 << 20)   /* the emulator's device memory is the host's */
+#else
+#define ALN_BUDGET ((i64)6 << 30)     /* the lanes' arenas, next to the index (K1 takes as much) */
+#endif
+#define ALN_T1_NODES 4096             /* queue nodes per lane in tier 1 (fewer if the lanes do not fit the budget) */
+#define ALN_T2_HITS 1024              /* tier 2: room for this many hits beyond max_entries + 9 queue entries, x4 per repeat at full size */
+
+/* A1 over all reads with small arenas (tier 1), then over the reads it listed with larger arenas (tier 2, fewer lanes: 16 times
+ * the nodes per round, up to max_entries + 9 entries and room for their hits), repeated while reads are listed (a full pool grows,
+ * a full-size arena too small for the hits gets more room); then the scan of the counts and A2 */
+extern "C" int bwag_aln(bwag_batch_t *b, const bwag_aln_par_t *par, bwag_aln_t *out)
+{
+	Lane *c = &b->lane;
+	CK(cudaSetDevice(b->ctx->device));
+	const int n = b->n;
+	memset(out, 0, sizeof(*out));
+	for (int r = 0; r < n; ++r)
+		if (b->h_off[r + 1] - b->h_off[r] >= 65536) return set_err("read %d of the batch has %lld bases; reads of 65536 bases or more are not supported", r, (long long)(b->h_off[r + 1] - b->h_off[r]));
+	if (par->s_mm < 0 || par->s_gapo < 0 || par->s_gape < 0) return set_err("negative penalties are not supported");
+	if (par->seed_len < 0) return set_err("the seed length must not be negative");
+	int md_max = 0;
+	for (int r = 0; r < n; ++r) if (par->max_diff[r] > md_max) md_max = par->max_diff[r];
+	/* every score pushed is below aln_score(max_diff+1, max_gapo+1, max_gape+1), the reference's number of stacks */
+	const i64 n_buckets = (i64)(md_max + 1) * par->s_mm + (i64)((par->max_gapo > 0 ? par->max_gapo : 0) + 1) * par->s_gapo + (i64)((par->max_gape > 0 ? par->max_gape : 0) + 1) * par->s_gape + 1;
+	if (n_buckets > (1 << 20)) return set_err("penalties too large: %lld queue scores", (long long)n_buckets);
+	const int seed_cap = par->seed_len < b->max_len ? par->seed_len : b->max_len;
+	const bool small = getenv("BWA_B200_TEST_SMALL_POOLS") != 0;   /* test hook: tier 1 and the pool too small for nearly every read */
+	i64 cap_pool = small ? n / 8 + 1 : 2 * (i64)n + 1024;
+	if (buf_reserve(&b->d_aln_md, (size_t)n + 16) || buf_reserve(&b->d_aln_n, 4 * ((size_t)n + 1)) || buf_reserve(&b->d_aln_beg, 8 * ((size_t)n + 1)) ||
+	    buf_reserve(&b->d_aln_redo[0], 4 * ((size_t)n + 1)) || buf_reserve(&b->d_aln_redo[1], 4 * ((size_t)n + 1)) || buf_reserve(&b->d_aln_off, 8 * ((size_t)n + 1)) ||
+	    buf_reserve(&b->d_aln_pool, sizeof(bwag_aln1_t) * (size_t)cap_pool) ||
+	    hbuf_reserve(&b->h_aln_n, 4 * ((size_t)n + 1)) || hbuf_reserve(&b->h_aln_off, 8 * ((size_t)n + 1))) return 1;
+	cap_pool = (i64)(b->d_aln_pool.cap / sizeof(bwag_aln1_t));
+	if (n) H2D(c, b->d_aln_md.p, par->max_diff, (size_t)n);
+	if (reset_counters(c)) return 1;
+	int grid_lanes = 2 * ALN_THREADS;
+#ifndef BWAG_CUSIM
+	{
+		int nb = 0;
+		CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_aln, ALN_THREADS, 0));
+		grid_lanes = b->ctx->n_sm * (nb > 0 ? nb : 1) * ALN_THREADS;
+	}
+#endif
+	AlnArgs a;
+	memset(&a, 0, sizeof(a));
+	a.codes = (const uint8_t *)b->d_codes.p; a.off = (const i64 *)b->d_off.p;
+	a.par = *par; a.par.max_diff = (const int8_t *)b->d_aln_md.p;
+	a.n_buckets = (int)n_buckets; a.max_len = b->max_len; a.seed_cap = seed_cap;
+	a.n_aln = (int *)b->d_aln_n.p; a.hit_beg = (i64 *)b->d_aln_beg.p;
+	a.n_pool = &c->d_cnt->aln_pool; a.n_redo = &c->d_cnt->aln_redo; a.flags = &c->d_cnt->aln_flags; a.next = &c->d_cnt->aln_next;
+	i64 cap_nodes = small ? 8 : ALN_T1_NODES, hit_room = ALN_T2_HITS;
+	int lanes = n < grid_lanes ? (n > 0 ? n : 1) : grid_lanes;
+	while (cap_nodes > 64 && lanes * aln_layout(a.n_buckets, a.max_len, seed_cap, cap_nodes).bytes > ALN_BUDGET) cap_nodes >>= 1;
+	const int *work = 0;
+	int n_work = n;
+	for (int round = 0;; ++round) {
+		const i64 lane_bytes = aln_layout(a.n_buckets, a.max_len, seed_cap, cap_nodes).bytes;
+		if (lanes > ALN_BUDGET / lane_bytes) lanes = (int)(ALN_BUDGET / lane_bytes);
+		if (lanes < 1) {
+			int r = 0;
+			if (work) CK(cudaMemcpy(&r, work, sizeof(int), cudaMemcpyDeviceToHost));
+			return set_err("read %d of the batch needs a search queue of %lld entries, more than the device can give", r, (long long)cap_nodes);
+		}
+		if (buf_reserve(&b->d_aln_arena, (size_t)(lanes * lane_bytes))) return 1;
+		a.work = work; a.n_work = n_work; a.arena = (unsigned char *)b->d_aln_arena.p; a.lane_bytes = lane_bytes;
+		a.cap_nodes = (int)cap_nodes; a.n_lanes = lanes;
+		a.pool = (bwag_aln1_t *)b->d_aln_pool.p; a.cap_pool = cap_pool;
+		a.redo = (int *)b->d_aln_redo[round & 1].p;
+		CK(cudaMemsetAsync(&c->d_cnt->aln_next, 0, sizeof(int), c->stream));
+		CK(cudaMemsetAsync(&c->d_cnt->aln_redo, 0, 2 * sizeof(u32), c->stream));
+		BWAG_LAUNCH(k_aln, (lanes + ALN_THREADS - 1) / ALN_THREADS, ALN_THREADS, 0, c->stream, c->ix, a);
+		CK(cudaGetLastError());
+		if (fetch_counters(c)) return 1;
+		++c->st.n_launch;
+		const u32 n_redo = c->h_cnt->aln_redo, flags = c->h_cnt->aln_flags;
+		if (round == 0) out->n_tier2 = n_redo;
+		if (n_redo == 0) break;
+		if (flags & 2) {   /* the pool is full: it grows, the hits already in it stay */
+			const i64 want = 2 * (i64)c->h_cnt->aln_pool + 1024;
+			if (buf_grow_keep(c, &b->d_aln_pool, sizeof(bwag_aln1_t) * (size_t)cap_pool, sizeof(bwag_aln1_t) * (size_t)want)) return 1;
+			cap_pool = (i64)(b->d_aln_pool.cap / sizeof(bwag_aln1_t));
+		}
+		/* tier 2 grows the arena 16-fold per round up to max_entries + 9 entries and the hit room: most listed reads need far
+		 * less than the full size, and smaller arenas leave room for more lanes */
+		const i64 queue_max = (i64)(par->max_entries > 0 ? par->max_entries : 0) + 9 + 1;
+		if (round > 0 && (flags & 1) && cap_nodes >= queue_max + hit_room) hit_room *= 4;   /* a full-size arena overflowed: only its hits can have done that */
+		cap_nodes = cap_nodes * 16 < queue_max + hit_room ? cap_nodes * 16 : queue_max + hit_room;
+		if (cap_nodes > 0x7fffffff) cap_nodes = 0x7fffffff;
+		work = (const int *)b->d_aln_redo[round & 1].p; n_work = (int)n_redo;
+		lanes = n_work < grid_lanes ? n_work : grid_lanes;
+	}
+	/* A2 */
+	BWAG_LAUNCH(k_fm_scan32, 1, FM_SCAN_THREADS, 0, c->stream, (const int *)b->d_aln_n.p, (i64)n, (i64 *)b->d_aln_off.p, &c->d_cnt->aln_total);
+	CK(cudaGetLastError());
+	if (fetch_counters(c)) return 1;
+	const i64 total = (i64)c->h_cnt->aln_total;
+	if (buf_reserve(&b->d_aln_out, sizeof(bwag_aln1_t) * ((size_t)total + 1)) || hbuf_reserve(&b->h_aln_out, sizeof(bwag_aln1_t) * ((size_t)total + 1))) return 1;
+	if (n) BWAG_LAUNCH(k_aln_gather, fm_grid(b->ctx, n), 128, 0, c->stream, n, (const int *)b->d_aln_n.p, (const i64 *)b->d_aln_beg.p, (const bwag_aln1_t *)b->d_aln_pool.p,
+	                   (const i64 *)b->d_aln_off.p, (bwag_aln1_t *)b->d_aln_out.p);
+	CK(cudaGetLastError());
+	c->st.n_launch += 2;
+	if (n) D2H(c, b->h_aln_n.p, b->d_aln_n.p, 4 * (size_t)n);
+	D2H(c, b->h_aln_off.p, b->d_aln_off.p, 8 * ((size_t)n + 1));
+	if (total) D2H(c, b->h_aln_out.p, b->d_aln_out.p, sizeof(bwag_aln1_t) * (size_t)total);
+	CK(stream_wait(c));
+	out->n_aln = (const int32_t *)b->h_aln_n.p; out->off = (const int64_t *)b->h_aln_off.p; out->aln = (const bwag_aln1_t *)b->h_aln_out.p;
+	return 0;
 }

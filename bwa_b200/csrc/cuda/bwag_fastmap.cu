@@ -13,6 +13,7 @@
  * a warp.  The scans are one block each (k_fm_scan); every buffer is sized from a scan's total, so nothing can overflow. */
 #include "bwag_dev.cuh"
 #include "bwag_kernels.h"
+#include "bwag_drv.h"
 
 /* exclusive prefix sum of in[0..n) into out[0..n], out[n] = *total = the sum; one block of FM_SCAN_THREADS, tiles of 4 per lane */
 template <typename T>
@@ -132,4 +133,72 @@ __global__ void k_fm_text(FmArgs a, int write)
 __global__ void k_fm_readoff(FmArgs a)
 {
 	for (int r = blockIdx.x * blockDim.x + threadIdx.x; r <= a.n_reads; r += gridDim.x * blockDim.x) a.toff[r] = a.tbeg[a.lbeg[r]];
+}
+
+/* ------------------------------------------------------------------------------------------------ host driver */
+
+/* K1 in its fastmap form, then F1-F3 with K2 between them; every buffer sized from a scan's total */
+extern "C" int bwag_fastmap(bwag_batch_t *b, const bwag_fastmap_par_t *par, bwag_fastmap_t *out)
+{
+	Lane *c = &b->lane;
+	const bwag_ctx_t *pc = b->ctx;
+	CK(cudaSetDevice(pc->device));
+	if (!pc->have_ctg) return set_err("bwag_fastmap needs the contig table (bwag_ctx_set_contigs)");
+	const int n = b->n;
+	for (int r = 0; r < n; ++r)
+		if (b->h_off[r + 1] - b->h_off[r] >= (1 << 23)) return set_err("read %d of the batch has %lld bases; reads of 2^23 bases or more are not supported", r, (long long)(b->h_off[r + 1] - b->h_off[r]));
+	bwag_seed_par_t sp;
+	memset(&sp, 0, sizeof(sp));
+	sp.min_seed_len = par->min_len;
+	const FmK1 fm = { par->min_intv < 1 ? 1 : par->min_intv, par->max_intv };
+	if (seed_impl(b, &sp, &fm, 0)) return 1;
+	const i64 n_lines = b->n_intv;
+	if (buf_reserve(&b->d_fm_lbeg, 8 * ((size_t)n + 1)) || buf_reserve(&b->d_fm_toff, 8 * ((size_t)n + 1)) ||
+	    buf_reserve(&b->d_fm_lines, sizeof(bwtintv_t) * ((size_t)n_lines + 1)) || buf_reserve(&b->d_fm_nrow, 8 * ((size_t)n_lines + 1)) ||
+	    buf_reserve(&b->d_fm_rbeg, 8 * ((size_t)n_lines + 1)) || buf_reserve(&b->d_fm_tlen, 8 * ((size_t)n_lines + 1)) || buf_reserve(&b->d_fm_tbeg, 8 * ((size_t)n_lines + 1)) ||
+	    hbuf_reserve(&b->h_fm_off, 8 * ((size_t)n + 1))) return 1;
+	FmArgs f;
+	memset(&f, 0, sizeof(f));
+	f.n_reads = n; f.n_lines = n_lines; f.max_iwidth = (u64)(i64)par->max_iwidth; f.ctg = pc->tctg;
+	f.intv_beg = (const i64 *)b->d_intv_beg.p; f.intv_n = (const int *)b->d_intv_n.p; f.intv = (const bwtintv_t *)b->d_intv.p;
+	f.lbeg = (const i64 *)b->d_fm_lbeg.p; f.lines = (bwtintv_t *)b->d_fm_lines.p; f.nrow = (i64 *)b->d_fm_nrow.p; f.rbeg = (const i64 *)b->d_fm_rbeg.p;
+	f.tlen = (i64 *)b->d_fm_tlen.p; f.tbeg = (const i64 *)b->d_fm_tbeg.p; f.toff = (i64 *)b->d_fm_toff.p;
+	/* F1: read order, rows wanted per line, their scan */
+	BWAG_LAUNCH(k_fm_scan32, 1, FM_SCAN_THREADS, 0, c->stream, (const int *)b->d_intv_n.p, (i64)n, (i64 *)b->d_fm_lbeg.p, &c->d_cnt->fm_total[0]);
+	BWAG_LAUNCH(k_fm_lines, fm_grid(b->ctx, n), 128, 0, c->stream, f);
+	BWAG_LAUNCH(k_fm_scan64, 1, FM_SCAN_THREADS, 0, c->stream, (const i64 *)b->d_fm_nrow.p, n_lines, (i64 *)b->d_fm_rbeg.p, &c->d_cnt->fm_total[1]);
+	CK(cudaGetLastError());
+	if (fetch_counters(c)) return 1;
+	c->st.n_launch += 3;
+	const i64 n_rows = (i64)c->h_cnt->fm_total[1];
+	/* F2 + K2: the rows, resolved in place */
+	if (buf_reserve(&b->d_fm_rows, 8 * ((size_t)n_rows + 1))) return 1;
+	f.rows = (i64 *)b->d_fm_rows.p;
+	if (n_rows > 0) {
+		BWAG_LAUNCH(k_fm_rows, fm_grid(b->ctx, n_lines), 128, 0, c->stream, f);
+		if (run_sa(b, f.rows, n_rows)) return 1;
+		c->st.n_launch += 2;
+	}
+	/* F3: line sizes, their scan, the text, each read's range */
+	BWAG_LAUNCH(k_fm_text, fm_grid(b->ctx, n_lines), 128, 0, c->stream, f, 0);
+	BWAG_LAUNCH(k_fm_scan64, 1, FM_SCAN_THREADS, 0, c->stream, (const i64 *)b->d_fm_tlen.p, n_lines, (i64 *)b->d_fm_tbeg.p, &c->d_cnt->fm_total[2]);
+	CK(cudaGetLastError());
+	if (fetch_counters(c)) return 1;
+	if (n_rows > 0) { c->st.ms_sa += elapsed_at(c, "sa", __FILE__, __LINE__); c->st.sa_touches += c->h_cnt->sa_touches; }
+	c->st.n_launch += 2;
+	const i64 n_text = (i64)c->h_cnt->fm_total[2];
+	if (buf_reserve(&b->d_fm_text, (size_t)n_text + 1) || hbuf_reserve(&b->h_fm_text, (size_t)n_text + 1)) return 1;
+	f.text = (char *)b->d_fm_text.p;
+	BWAG_LAUNCH(k_fm_text, fm_grid(b->ctx, n_lines), 128, 0, c->stream, f, 1);
+	BWAG_LAUNCH(k_fm_readoff, fm_grid(b->ctx, (i64)n + 1), 128, 0, c->stream, f);
+	CK(cudaGetLastError());
+	c->st.n_launch += 2;
+	CK(cudaEventRecord(c->ev0, c->stream));
+	if (n_text) D2H(c, b->h_fm_text.p, b->d_fm_text.p, (size_t)n_text);
+	D2H(c, b->h_fm_off.p, b->d_fm_toff.p, 8 * ((size_t)n + 1));
+	CK(cudaEventRecord(c->ev1, c->stream));
+	CK(stream_wait(c));
+	c->st.ms_d2h += elapsed_at(c, "d2h", __FILE__, __LINE__);
+	out->text = (const char *)b->h_fm_text.p; out->off = (const int64_t *)b->h_fm_off.p;
+	return 0;
 }

@@ -15,12 +15,7 @@
  * Then the Occ checkpoints every 128 symbols are counted, scanned and interleaved with the symbols (bwt_bwtupdate_core,
  * bwtindex.c:150-172).  Device memory: the packed text (n/4 bytes), one byte per BWT row, the SA sample (n/4 bytes) and one
  * group's working set; nothing of 8 bytes per suffix over the whole text. */
-#include <stdio.h>
-#include <stdlib.h>
-#include <string.h>
-#include <stdarg.h>
-#include "bwag_dev.cuh"
-#include "bwag_kernels.h"
+#include "bwag_drv.h"
 
 #define IX_HIST_BASES 6          /* buckets of the planning histogram: 4^6, 16 KB of shared counters */
 #define IX_THREADS 256
@@ -29,17 +24,8 @@
 #define IX_GROUP_BYTES 56        /* working set per suffix of a group: keys and positions twice, tie lists, run table */
 #define IX_SA_INTV 32
 
-static int ix_err(const char *fmt, ...)   /* the message goes to bwag_last_error() */
-{
-	char msg[512];
-	va_list ap;
-	va_start(ap, fmt);
-	vsnprintf(msg, sizeof(msg), fmt, ap);
-	va_end(ap);
-	return bwag_set_error(msg);
-}
 static int ix_clz64_host(u64 x) { return x ? __builtin_clzll(x) : 64; }
-#define IXCK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { rc = ix_err("%s failed at %s:%d: %s", #call, __FILE__, __LINE__, cudaGetErrorString(e_)); goto done; } } while (0)
+#define IXCK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { rc = set_err("%s failed at %s:%d: %s", #call, __FILE__, __LINE__, cudaGetErrorString(e_)); goto done; } } while (0)
 
 /* ------------------------------------------------------------------------------------------------ device helpers */
 
@@ -346,15 +332,15 @@ extern "C" int bwag_index_build(int device, const uint8_t *pac, int64_t l_pac, b
 	const char *env = getenv("BWA_B200_INDEX_BUCKET_BASES"), *genv = getenv("BWA_B200_INDEX_GROUP_SUFFIXES");
 	g_ix_cur = g_ix_peak = 0;
 	memset(out, 0, sizeof(*out));
-	if (l_pac <= 0) return ix_err("empty reference");
-	if (n >= (u64)BWAG_MAX_SB << BWAG_SB_SHIFT) return ix_err("reference too large: %llu bases", (unsigned long long)l_pac);
+	if (l_pac <= 0) return set_err("empty reference");
+	if (n >= (u64)BWAG_MAX_SB << BWAG_SB_SHIFT) return set_err("reference too large: %llu bases", (unsigned long long)l_pac);
 	if (env && *env) {
 		kb = atoi(env); forced = 1;
-		if (kb < 1 || kb > IX_HIST_BASES) return ix_err("BWA_B200_INDEX_BUCKET_BASES must lie in 1..%d", IX_HIST_BASES);
+		if (kb < 1 || kb > IX_HIST_BASES) return set_err("BWA_B200_INDEX_BUCKET_BASES must lie in 1..%d", IX_HIST_BASES);
 	}
 	{
 		int ndev = 0;
-		if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return ix_err("no CUDA device is visible: this library has no CPU path");
+		if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return set_err("no CUDA device is visible: this library has no CPU path");
 	}
 	if (device < 0) IXCK(cudaGetDevice(&device));
 	IXCK(cudaSetDevice(device));
@@ -370,7 +356,7 @@ extern "C" int bwag_index_build(int device, const uint8_t *pac, int64_t l_pac, b
 	{
 		const double fixed = (double)nw * 4 + (double)(n + 1) + (double)n_sa * 8 + (double)(l_pac / 4 + 1);
 		if (fixed + (double)(64u << 20) > 0.9 * (double)free_b)
-			return ix_err("not enough free device memory: the text, BWT and SA sample of %llu bases need %.2f GB, %.2f GB are free",
+			return set_err("not enough free device memory: the text, BWT and SA sample of %llu bases need %.2f GB, %.2f GB are free",
 			              (unsigned long long)n, fixed / 1e9, (double)free_b / 1e9);
 	}
 	IXCK(ix_malloc((void **)&W, nw * 4));
@@ -395,18 +381,18 @@ extern "C" int bwag_index_build(int device, const uint8_t *pac, int64_t l_pac, b
 	ix_free(hist, ((u64)1 << (2 * kb)) * 8); hist = 0;
 	IXCK(cudaMemGetInfo(&free_b, &total_b));   /* again: others may have taken memory since the first look */
 	if (0.9 * (double)free_b < (double)(64u << 20) + IX_GROUP_BYTES)
-		{ rc = ix_err("not enough free device memory: %.2f GB are free beside the text, BWT and SA sample", (double)free_b / 1e9); goto done; }
+		{ rc = set_err("not enough free device memory: %.2f GB are free beside the text, BWT and SA sample", (double)free_b / 1e9); goto done; }
 	cap = (u64)((0.9 * (double)free_b - (double)(64u << 20)) / IX_GROUP_BYTES);
 	if (genv && *genv) {   /* tests: several groups of many buckets on a small reference */
 		const long long g = atoll(genv);
-		if (g < 1) { rc = ix_err("BWA_B200_INDEX_GROUP_SUFFIXES must be positive"); goto done; }
+		if (g < 1) { rc = set_err("BWA_B200_INDEX_GROUP_SUFFIXES must be positive"); goto done; }
 		if ((u64)g < cap) cap = (u64)g;
 	}
 	{
 		u64 acc = 0;
 		for (u32 b = 0; b < (1u << (2 * kb)); ++b) {
 			if (h_hist[b] > cap)
-				{ rc = ix_err("not enough free device memory: the %llu suffixes of one bucket need %.2f GB, %.2f GB are free (or more than BWA_B200_INDEX_GROUP_SUFFIXES)",
+				{ rc = set_err("not enough free device memory: the %llu suffixes of one bucket need %.2f GB, %.2f GB are free (or more than BWA_B200_INDEX_GROUP_SUFFIXES)",
 				              (unsigned long long)h_hist[b], (double)h_hist[b] * IX_GROUP_BYTES / 1e9, (double)free_b / 1e9); goto done; }
 			if (forced || acc + h_hist[b] > cap) acc = 0;
 			acc += h_hist[b];
@@ -442,7 +428,7 @@ extern "C" int bwag_index_build(int device, const uint8_t *pac, int64_t l_pac, b
 		BWAG_LAUNCH(k_ix_list, ix_grid(n, n_sm), IX_THREADS, 0, 0, W, n, kb, lo, hi, keys0, pos0, dcnt);
 		IXCK(cudaGetLastError());
 		IXCK(cudaMemcpy(h_cnt, dcnt, 8, cudaMemcpyDeviceToHost));
-		if (h_cnt[0] != m) { rc = ix_err("bucket listing found %llu suffixes, expected %llu", (unsigned long long)h_cnt[0], (unsigned long long)m); goto done; }
+		if (h_cnt[0] != m) { rc = set_err("bucket listing found %llu suffixes, expected %llu", (unsigned long long)h_cnt[0], (unsigned long long)m); goto done; }
 		/* 2. radix sort on the bits that vary within the group */
 		u64 *kin = keys0, *kout = keys1, *vin = pos0, *vout = pos1;
 		{
@@ -483,7 +469,7 @@ extern "C" int bwag_index_build(int device, const uint8_t *pac, int64_t l_pac, b
 		row += m;
 		lo = hi;
 	}
-	if (row != n + 1) { rc = ix_err("sorted %llu rows, expected %llu", (unsigned long long)row, (unsigned long long)n + 1); goto done; }
+	if (row != n + 1) { rc = set_err("sorted %llu rows, expected %llu", (unsigned long long)row, (unsigned long long)n + 1); goto done; }
 	IXCK(cudaMemcpy(&primary, dcnt + 3, 8, cudaMemcpyDeviceToHost));
 	ix_free(keys0, max_group * 8); ix_free(keys1, max_group * 8); ix_free(pos0, max_group * 8); ix_free(pos1, max_group * 8);
 	ix_free(bh, nblk_cap * 256 * 8); ix_free(run_start, max_group / 2 * 8); ix_free(run_len, max_group / 2 * 8); ix_free(run_off, max_group / 2 * 8);
@@ -503,7 +489,7 @@ extern "C" int bwag_index_build(int device, const uint8_t *pac, int64_t l_pac, b
 	for (int k = 0; k < 4; ++k) IXCK(cudaMemcpy(&h_cnt[k], occ + (u64)k * (n_blk + 1) + n_blk, 8, cudaMemcpyDeviceToHost));
 	out->bwt = (uint32_t *)malloc(bwt_words * 4);
 	out->sa = (uint64_t *)malloc(n_sa * 8);
-	if (!out->bwt || !out->sa) { rc = ix_err("out of host memory"); goto done; }
+	if (!out->bwt || !out->sa) { rc = set_err("out of host memory"); goto done; }
 	IXCK(cudaMemcpy(out->bwt, obwt, bwt_words * 4, cudaMemcpyDeviceToHost));
 	IXCK(cudaMemcpy(out->sa, SA, n_sa * 8, cudaMemcpyDeviceToHost));
 	out->max_group = max_group;

@@ -33,8 +33,6 @@
 
 struct Intv;
 
-int bwag_set_error(const char *msg);   /* sets what bwag_last_error() returns; returns 1 */
-
 struct SeedArgs {
 	/* batch */
 	const uint8_t *codes; const i64 *off; int n_reads;

@@ -14,6 +14,7 @@
  * gives inf or NaN there as on the host) and uint8_t arithmetic for the qualities. */
 #include "bwag_dev.cuh"
 #include "bwag_kernels.h"
+#include "bwag_drv.h"
 
 #define PEM_RATIO ((double)0.9f)   /* MAX_SCORE_RATIO (pemerge.c:19), a float compared with doubles */
 #define PEM_A 5                     /* the reference's fixed scoring: bwa_fill_scmat(5, 4), N scores -1 */
@@ -192,4 +193,79 @@ __global__ void k_pem_text(PemArgs a, int write)
 		__syncthreads();
 		if (threadIdx.x < 9 && cnt[threadIdx.x]) atomicAdd(&a.cnt[threadIdx.x], (u64)cnt[threadIdx.x]);
 	}
+}
+
+/* ------------------------------------------------------------------------------------------------ host driver */
+
+/* M1, K6, M2/M3, then M4 around a scan */
+extern "C" int bwag_pemerge(bwag_batch_t *b, const bwag_pemerge_par_t *par, bwag_pemerge_t *out)
+{
+	Lane *c = &b->lane;
+	CK(cudaSetDevice(b->ctx->device));
+	memset(out, 0, sizeof(*out));
+	const int n = b->n;
+	if (n & 1) return set_err("bwag_pemerge: a batch of %d reads is not a batch of pairs", n);
+	const int np = n >> 1;
+	const i64 nb = b->total_bases, nn = par->name_off[n];
+	int max_q = 16, max_t = 16;
+	for (int i = 0; i < np; ++i) {
+		const int l0 = (int)(b->h_off[2 * i + 1] - b->h_off[2 * i]), l1 = (int)(b->h_off[2 * i + 2] - b->h_off[2 * i + 1]);
+		if (l0 > max_t) max_t = l0;
+		if (l1 > max_q) max_q = l1;
+	}
+	if (buf_reserve(&b->d_pm_qual, (size_t)nb + 16) || buf_reserve(&b->d_pm_hasq, (size_t)n + 16) || buf_reserve(&b->d_pm_names, (size_t)nn + 16) ||
+	    buf_reserve(&b->d_pm_noff, 8 * ((size_t)n + 1)) || buf_reserve(&b->d_swpool, (size_t)nb + 16) || buf_reserve(&b->d_pm_q, (size_t)nb + 16) ||
+	    buf_reserve(&b->d_swtasks, sizeof(bwag_swtask_t) * ((size_t)np + 1)) || buf_reserve(&b->d_pm_code, (size_t)np + 16) || buf_reserve(&b->d_pm_ovl, 4 * ((size_t)np + 1)) ||
+	    buf_reserve(&b->d_pm_tlen, 8 * ((size_t)np + 1)) || buf_reserve(&b->d_pm_tbeg, 8 * ((size_t)np + 1)) || buf_reserve(&b->d_pm_cnt, 8 * 9) ||
+	    hbuf_reserve(&b->h_pm_cnt, 8 * 9)) return 1;
+	PemArgs a;
+	memset(&a, 0, sizeof(a));
+	a.n_pairs = np; a.T = par->T; a.q_thres = par->q_thres; a.q_def = par->q_def; a.flag = par->flag;
+	a.raw = (const uint8_t *)b->d_codes.p; a.off = (const i64 *)b->d_off.p;
+	a.qual = (const uint8_t *)b->d_pm_qual.p; a.has_qual = (const uint8_t *)b->d_pm_hasq.p;
+	a.names = (const char *)b->d_pm_names.p; a.name_off = (const i64 *)b->d_pm_noff.p;
+	a.s = (uint8_t *)b->d_swpool.p; a.q = (uint8_t *)b->d_pm_q.p; a.tasks = (bwag_swtask_t *)b->d_swtasks.p;
+	a.code = (int8_t *)b->d_pm_code.p; a.ovl = (int *)b->d_pm_ovl.p;
+	a.tlen = (i64 *)b->d_pm_tlen.p; a.tbeg = (const i64 *)b->d_pm_tbeg.p; a.cnt = (u64 *)b->d_pm_cnt.p;
+	if (reset_counters(c)) return 1;
+	if (nb) H2D(c, b->d_pm_qual.p, par->qual, (size_t)nb);
+	if (n) H2D(c, b->d_pm_hasq.p, par->has_qual, (size_t)n);
+	if (nn) H2D(c, b->d_pm_names.p, par->names, (size_t)nn);
+	H2D(c, b->d_pm_noff.p, par->name_off, 8 * ((size_t)n + 1));
+	CK(cudaMemsetAsync(b->d_pm_cnt.p, 0, 8 * 9, c->stream));
+	if (np) BWAG_LAUNCH(k_pem_encode, fm_grid(b->ctx, np), 128, 0, c->stream, a);
+	CK(cudaGetLastError());
+	++c->st.n_launch;
+	if (par->merge && np) {
+		bwag_sw_par_t sp;   /* ksw_align(l2, s1, l1, s0, 5, bwa_fill_scmat(5, 4), 2, 17, xtra): the same gaps for deletions and insertions */
+		memset(&sp, 0, sizeof(sp));
+		sp.a = 5; sp.b = 4; sp.o_del = sp.o_ins = 2; sp.e_del = sp.e_ins = 17;
+		for (int i = 0; i < 5; ++i) for (int j = 0; j < 5; ++j) sp.mat[i * 5 + j] = (int8_t)(i < 4 && j < 4 ? (i == j ? 5 : -4) : -1);
+		if (localsw_on_device(b, &sp, np, max_q, max_t)) return 1;
+		a.res = (const bwag_swres_t *)b->d_swres.p;
+		const i64 blocks = ((i64)np + 3) / 4, cap = (i64)b->ctx->n_sm * 16;
+		BWAG_LAUNCH(k_pem_decide, (int)(blocks < cap ? blocks : cap), 128, 0, c->stream, a);
+		CK(cudaGetLastError());
+		if (fetch_counters(c)) return 1;
+		c->st.ms_localsw += elapsed_at(c, "localsw", __FILE__, __LINE__); c->st.n_launch += 2; c->st.sw_tasks += (u64)np;
+		if (c->h_cnt->flags & 32u) return set_err("pemerge: a local alignment exceeded the scratch capacity");
+	}
+	/* M4: sizes, their scan, then the text */
+	if (np) BWAG_LAUNCH(k_pem_text, fm_grid(b->ctx, np), 128, 0, c->stream, a, 0);
+	BWAG_LAUNCH(k_fm_scan64, 1, FM_SCAN_THREADS, 0, c->stream, (const i64 *)b->d_pm_tlen.p, (i64)np, (i64 *)b->d_pm_tbeg.p, &c->d_cnt->pm_total);
+	CK(cudaGetLastError());
+	if (fetch_counters(c)) return 1;
+	c->st.n_launch += 2;
+	const i64 n_text = (i64)c->h_cnt->pm_total;
+	if (buf_reserve(&b->d_pm_text, (size_t)n_text + 16) || hbuf_reserve(&b->h_pm_text, (size_t)n_text + 16)) return 1;
+	a.text = (char *)b->d_pm_text.p;
+	if (np) BWAG_LAUNCH(k_pem_text, fm_grid(b->ctx, np), 128, 0, c->stream, a, 1);
+	CK(cudaGetLastError());
+	++c->st.n_launch;
+	if (n_text) D2H(c, b->h_pm_text.p, b->d_pm_text.p, (size_t)n_text);
+	D2H(c, b->h_pm_cnt.p, b->d_pm_cnt.p, 8 * 9);
+	CK(stream_wait(c));
+	out->text = (const char *)b->h_pm_text.p; out->n_text = n_text;
+	memcpy(out->cnt, b->h_pm_cnt.p, 8 * 9);
+	return 0;
 }

@@ -4,7 +4,7 @@ time two or more lanes had a stage running, and where the idle gaps are.
 
     BWA_B200_GPUTRACE=1 python bench.py --worker ... 2> run.err;  python tools/gpu_timeline.py run.err [skip_ms]
 
-Each `[gputrace] <lane> <source line> <t0> <t1>` line is one timed stage (kernel(s) or copy between two CUDA events of one lane's
+Each `[gputrace] <lane> <stage:file:line> <t0> <t1>` line is one timed stage (kernel(s) or copy between two CUDA events of one lane's
 stream), in ms on the device clock.  A stage's interval includes the time its kernels waited behind other streams' kernels, so
 "sum of stages" exceeds wall time when lanes compete; "union" is the time at least one lane had a stage open."""
 import collections
@@ -57,7 +57,7 @@ def main():
     for a, b, _, ln in iv:
         by[ln][0] += 1
         by[ln][1] += b - a
-    print("by stage (counter the timer adds to : its line in bwag_api.cu): count, total ms, mean ms")
+    print("by stage (counter the timer adds to : the driver file and line of the timer): count, total ms, mean ms")
     for ln, (n, tot) in sorted(by.items(), key=lambda kv: -kv[1][1]):
         print("  %-16s %6d %10.1f %8.3f" % (ln, n, tot, tot / n))
     gaps.sort(reverse=True)
