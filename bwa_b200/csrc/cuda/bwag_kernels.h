@@ -53,6 +53,9 @@ struct SeedArgs {
 	i64 cap_intv, cap_seeds;
 	/* counters: [0] next read, n_intv, n_seeds, occ touches, flags */
 	int *next_read; u64 *n_intv; u64 *n_seeds; u64 *occ_touches; u32 *flags;
+#ifdef BWAG_K1_CLOCKS
+	u64 *k1clk;   /* BWAG_K1CLK_LANE_WORDS counters of k_smem_c (include/bwa_b200_dev.h) */
+#endif
 };
 
 struct SaArgs { i64 *rbeg; i64 n; u64 *next; u64 *sa_touches; };

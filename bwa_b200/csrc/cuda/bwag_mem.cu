@@ -27,6 +27,24 @@ extern "C" int bwag_k3_clocks(uint64_t *out, int reset)
 	return -1;
 #endif
 }
+/* K1 counters of a build with -DBWAG_K1_CLOCKS (tools/k1_bench.py): BWAG_K1CLK_WORDS words, include/bwa_b200_dev.h */
+#ifdef BWAG_K1_CLOCKS
+static pthread_mutex_t g_k1clk_mu = PTHREAD_MUTEX_INITIALIZER;
+static u64 g_k1clk[BWAG_K1CLK_WORDS];
+#endif
+extern "C" int bwag_k1_clocks(uint64_t *out, int reset)
+{
+#ifdef BWAG_K1_CLOCKS
+	pthread_mutex_lock(&g_k1clk_mu);
+	if (out) memcpy(out, g_k1clk, sizeof(g_k1clk));
+	if (reset) memset(g_k1clk, 0, sizeof(g_k1clk));
+	pthread_mutex_unlock(&g_k1clk_mu);
+	return 0;
+#else
+	(void)out; (void)reset;
+	return -1;
+#endif
+}
 #ifdef BWAG_K3_CLOCKS
 static void k3clk_add(const u32 *rec, int n)
 {
@@ -139,6 +157,12 @@ int seed_impl(bwag_batch_t *b, const bwag_seed_par_t *par, const FmK1 *fm, bwag_
 		a.cap_intv = cap_intv; a.cap_seeds = cap_seeds;
 		a.next_read = &c->d_cnt->next_read; a.n_intv = &c->d_cnt->n_intv; a.n_seeds = &c->d_cnt->n_seeds; a.occ_touches = &c->d_cnt->occ_touches; a.flags = &c->d_cnt->flags;
 		if (reset_counters(c)) return 1;
+#ifdef BWAG_K1_CLOCKS   /* K1f and k_smem_c timed apart, and k_smem_c's counters */
+		cudaEvent_t k1e[2];
+		for (int e = 0; e < 2; ++e) CK(cudaEventCreate(&k1e[e]));
+		CK(cudaMalloc((void **)&a.k1clk, 8 * BWAG_K1CLK_LANE_WORDS));
+		CK(cudaMemsetAsync(a.k1clk, 0, 8 * BWAG_K1CLK_LANE_WORDS, c->stream));
+#endif
 		CK(cudaEventRecord(c->ev0, c->stream));
 		if (want_pack) {   /* the packed copies K1's table lookups key on, and which reads have an ambiguous base */
 			a.packed = (const u32 *)c->s_pack.p; a.nmask = nstride ? (const u32 *)c->s_pack.p + pack_words : 0; a.hasn = (const u32 *)c->s_pack.p + pack_words + nmask_words;
@@ -146,6 +170,9 @@ int seed_impl(bwag_batch_t *b, const bwag_seed_par_t *par, const FmK1 *fm, bwag_
 			CK(cudaGetLastError());
 			++c->st.n_launch;
 		}
+#ifdef BWAG_K1_CLOCKS
+		CK(cudaEventRecord(k1e[0], c->stream));
+#endif
 		if (a.n3) {   /* third pass first: K1 appends its seeds to the read's list */
 			int g3 = b->ctx->grid_k1f;
 			if (g3 > (n + K1F_THREADS - 1) / K1F_THREADS) g3 = (n + K1F_THREADS - 1) / K1F_THREADS;
@@ -153,6 +180,9 @@ int seed_impl(bwag_batch_t *b, const bwag_seed_par_t *par, const FmK1 *fm, bwag_
 			CK(cudaGetLastError());
 			++c->st.n_launch;
 		}
+#ifdef BWAG_K1_CLOCKS
+		CK(cudaEventRecord(k1e[1], c->stream));
+#endif
 #ifndef K1_PACKED8
 		if (k1c) BWAG_LAUNCH(k_smem_c, grid, K1_THREADS, smem, c->stream, c->ix, a);
 		else
@@ -168,6 +198,23 @@ int seed_impl(bwag_batch_t *b, const bwag_seed_par_t *par, const FmK1 *fm, bwag_
 		}
 		if (fetch_counters(c)) return 1;
 		c->st.ms_smem += elapsed_at(c, "smem", __FILE__, __LINE__); c->st.n_launch += 2;
+#ifdef BWAG_K1_CLOCKS
+		{
+			u64 h[BWAG_K1CLK_LANE_WORDS];
+			float ms_f = 0, ms_c = 0;
+			CK(cudaMemcpy(h, a.k1clk, sizeof(h), cudaMemcpyDeviceToHost));
+			CK(cudaEventElapsedTime(&ms_f, k1e[0], k1e[1])); CK(cudaEventElapsedTime(&ms_c, k1e[1], c->ev1));
+			CK(cudaFree(a.k1clk));
+			a.k1clk = 0;
+			for (int e = 0; e < 2; ++e) cudaEventDestroy(k1e[e]);
+			if (k1c) {
+				pthread_mutex_lock(&g_k1clk_mu);
+				for (int w = 0; w < BWAG_K1CLK_LANE_WORDS; ++w) g_k1clk[w] += h[w];
+				g_k1clk[BWAG_K1CLK_K1F_NS] += (u64)(ms_f * 1e6); g_k1clk[BWAG_K1CLK_K1C_NS] += (u64)(ms_c * 1e6); g_k1clk[BWAG_K1CLK_CALLS] += 1;
+				pthread_mutex_unlock(&g_k1clk_mu);
+			}
+		}
+#endif
 		if (!(c->h_cnt->flags & 41u)) break;
 		if (attempt >= 6) return set_err("seeding: output pools keep overflowing (intervals %llu, seeds %llu)", (unsigned long long)c->h_cnt->n_intv, (unsigned long long)c->h_cnt->n_seeds);
 		if (c->h_cnt->flags & 1u) { /* pools too small: the counters say how much is needed */

@@ -658,6 +658,33 @@ k_smem_fm(DevIndex ix, SeedArgs a, int min_intv, u64 max_intv)
 #define CENT_LD(l, idx, X0, X1, X2, E) do { const int l_ = (l), i_ = (idx); ulonglong2 v_; ENT_COUNT(i_ < K1C_SLOTS ? 0 : i_); \
 		if (i_ < K1C_SLOTS) v_ = sl[(l_ * K1C_SLOTS + i_) * nthr]; else v_ = gl[l_ * a.cap_list + i_]; unpack_ent(v_, X0, X1, X2, E); } while (0)
 
+/* the second lookup of a pair: one 16-byte table entry */
+__device__ __forceinline__ uint4 ld_ktab_ent(const ulonglong2 *p)
+{
+#ifdef BWAG_CUSIM
+	__atomic_fetch_add(&bwag_cusim_sector_loads, 1ull, __ATOMIC_RELAXED);
+#endif
+	return __ldg(reinterpret_cast<const uint4 *>(p));
+}
+/* Occ-block touches of bwt_extend on the interval (xs, e2) as the reference counts them, with no load: extend_step3's t12 */
+__device__ __forceinline__ int ref_touches(const DevIndex &ix, u64 xs, u64 e2)
+{
+	const u64 k = xs - 1, l = xs - 1 + e2;
+	const bool kv = k != (u64)-1, lv = l != (u64)-1;
+	const u64 kp = k - (k >= ix.primary), lp = l - (l >= ix.primary);
+	return (kv && lv && (kp >> 7) == (lp >> 7)) ? 1 : 2;
+}
+#ifdef BWAG_K1_CLOCKS   /* tools/k1_bench.py: per-lane counts (the BWAG_K1CLK_* words) summed into a.k1clk; compiles to nothing otherwise */
+#define K1CLK(w_, v_) (clk[w_] += (u64)(v_))
+#ifdef BWAG_CUSIM
+#define K1NOW() 0ull
+#else
+#define K1NOW() ((u64)clock64())
+#endif
+#else
+#define K1CLK(w_, v_) ((void)0)
+#endif
+
 __global__ void __launch_bounds__(K1_THREADS, K1_MIN_BLOCKS)
 k_smem_c(DevIndex ix, SeedArgs a)
 {
@@ -687,6 +714,10 @@ k_smem_c(DevIndex ix, SeedArgs a)
 	int pl = 0;
 	u32 cm = 0, rm = 0;            /* short candidates: of the list being built / still to visit in this step */
 	bool cur_short = false;        /* the candidate being extended came from the mask: e0..e2 are stale */
+	u32 pend2 = 0;                 /* a backward pair: the end of the second mask candidate */
+#ifdef BWAG_K1_CLOCKS
+	u64 clk[BWAG_K1CLK_LANE_WORDS] = {};
+#endif
 	const uint8_t *q = 0;
 	u64 ik0 = 0, ik1 = 0, ik2 = 0, curr_last_x2 = 0;
 	u32 ikend = 0, pend = 0;
@@ -695,8 +726,9 @@ k_smem_c(DevIndex ix, SeedArgs a)
 	u32 overflow = 0;
 
 	for (;;) {
-		bool need = false;
+		bool need = false, two = false;   /* two: this extension and the lane's next one are both table lookups, issued together */
 		int back = 0;
+		K1CLK(BWAG_K1CLK_ITERS, 1);
 		for (;;) {
 			if (st == ST_IDLE) {
 				if (pass == 0) {
@@ -714,6 +746,9 @@ k_smem_c(DevIndex ix, SeedArgs a)
 					}
 					if (!found) { pass = 2; continue; }
 				} else {
+#ifdef BWAG_K1_CLOCKS
+					const u64 t_turn = K1NOW();
+#endif
 					if (rid >= 0) {
 						const int n3 = a.n3 ? a.n3[rid] : 0;
 						const i64 base = (i64)atomicAdd(a.n_intv, (u64)(mem_n + n3));
@@ -732,7 +767,7 @@ k_smem_c(DevIndex ix, SeedArgs a)
 						}
 					}
 					rid = atomicAdd(a.next_read, 1);
-					if (rid >= a.n_reads) { rid = -1; st = ST_NONE; break; }
+					if (rid >= a.n_reads) { rid = -1; st = ST_NONE; K1CLK(BWAG_K1CLK_TURN_CYC, K1NOW() - t_turn); break; }
 					const i64 o = a.off[rid];
 					len = (int)(a.off[rid + 1] - o);
 					pass = 0; x = 0; mem_n = 0;
@@ -746,6 +781,7 @@ k_smem_c(DevIndex ix, SeedArgs a)
 							for (int w = 0; w < nwp; ++w) sp_sh[w] = gp[w];
 						} else spg = gp;
 					}
+					K1CLK(BWAG_K1CLK_TURN_CYC, K1NOW() - t_turn); K1CLK(BWAG_K1CLK_READS, 1);
 					continue;
 				}
 				INIT_INTV(CQBASE(sx), ik0, ik1, ik2);
@@ -754,7 +790,11 @@ k_smem_c(DevIndex ix, SeedArgs a)
 				continue;
 			}
 			if (st == ST_FWD) {
-				if (i < len && !CQISN(i)) { e0 = ik0; e1 = ik1; e2 = ik2; need = true; back = 0; cur_short = false; break; }
+				if (i < len && !CQISN(i)) {
+					e0 = ik0; e1 = ik1; e2 = ik2; need = true; back = 0; cur_short = false;
+					two = i + 2 - sx <= ktk && i + 1 < len && !CQISN(i + 1);   /* q[sx..i] and q[sx..i+1] */
+					break;
+				}
 				PUSH_CAND((int)ikend - sx + 1, ik0, ik1, ik2, ikend);
 				TURN_AROUND();
 				continue;
@@ -782,6 +822,8 @@ k_smem_c(DevIndex ix, SeedArgs a)
 					const int b = 31 - __clz(rm);
 					rm ^= 1u << b;
 					pend = (u32)(sx + 1 + b);
+					two = rm != 0;         /* the next candidate in visiting order is a mask bit too */
+					if (two) { const int b2 = 31 - __clz(rm); rm ^= 1u << b2; pend2 = (u32)(sx + 1 + b2); }
 					cur_short = true; need = true; back = 1;
 					break;
 				}
@@ -798,6 +840,7 @@ k_smem_c(DevIndex ix, SeedArgs a)
 
 		const int cq = CQBASE(i);
 		u64 o_s, o_o, o_x2;
+		uint4 ev2 = make_uint4(0, 0, 0, 0);
 		{
 			const int rlen = back ? (int)pend - i : i + 1 - sx;
 			const bool tab = rlen <= ktk;
@@ -807,39 +850,64 @@ k_smem_c(DevIndex ix, SeedArgs a)
 				const int pos = back ? i : sx;
 				const u32 win = __funnelshift_r(SPW(pos >> 4), SPW((pos >> 4) + 1), (u32)(pos & 15) << 1);
 				tidx = ktab_off(rlen) + (win & ((1u << (2 * rlen)) - 1u));
+				if (two) {                  /* same start: the forward string one base longer, or the next candidate's q[i..pend2) */
+					const int rlen2 = back ? (int)pend2 - i : rlen + 1;
+					ev2 = ld_ktab_ent(ix.ktab + ktab_off(rlen2) + (win & ((1u << (2 * rlen2)) - 1u)));
+				}
 			}
 			/* a candidate from the mask passes stale (valid) interval registers; its lane is a table lane, which ignores them */
 			extend_step3(ix, back ? e0 : e1, back ? e1 : e0, e2, back ? cq : 3 - cq, tab, tidx, back, t12, o_s, o_o, o_x2, ct);
 			touches += cur_short ? (u64)(1u + (ct >> KTAB_BT_SHIFT)) : (u64)t12;
+			K1CLK(back ? (cur_short ? BWAG_K1CLK_BWD_MASK : BWAG_K1CLK_BWD_LIST) : (tab ? BWAG_K1CLK_FWD_TAB : BWAG_K1CLK_FWD_OCC), 1);
+			K1CLK(back ? BWAG_K1CLK_PAIR_BWD : BWAG_K1CLK_PAIR_FWD, two);
 		}
 
-		if (st == ST_FWD) {                 /* bwt.c:307-316 */
-			bool stop = false;
-			if (o_x2 != ik2) {
-				PUSH_CAND((int)ikend - sx + 1, ik0, ik1, ik2, ikend);
-				if (o_x2 < (u64)min_intv) stop = true;
-			}
-			if (stop) TURN_AROUND();
-			else {
-				ik0 = o_o; ik1 = o_s; ik2 = o_x2; ikend = (u32)i + 1;
-				++i;
-				if (i == len) {
+		/* the result, then that of the pair's second lookup: the reference's bookkeeping sees them in visiting order */
+		for (;;) {
+			if (st == ST_FWD) {                 /* bwt.c:307-316 */
+				bool stop = false;
+				if (o_x2 != ik2) {
 					PUSH_CAND((int)ikend - sx + 1, ik0, ik1, ik2, ikend);
-					TURN_AROUND();
+					if (o_x2 < (u64)min_intv) stop = true;
 				}
-			}
-		} else {                            /* ST_BWD, bwt.c:331-343 */
-			const bool first = n_curr == 0 && cm == 0;
-			if (o_x2 < (u64)min_intv) {
-				if (first && (m1_n == 0 || i + 1 < last_start)) {
-					if (!cur_short) EMIT(e0, e1, e2, i + 1, pend);
-					++m1_n; last_start = i + 1;
+				if (stop) TURN_AROUND();
+				else {
+					ik0 = o_o; ik1 = o_s; ik2 = o_x2; ikend = (u32)i + 1;
+					++i;
+					if (i == len) {
+						PUSH_CAND((int)ikend - sx + 1, ik0, ik1, ik2, ikend);
+						TURN_AROUND();
+					}
 				}
-			} else if (first || o_x2 != curr_last_x2) {
-				PUSH_CAND((int)pend - i + 1, o_s, o_o, o_x2, pend);
-				curr_last_x2 = o_x2;
+			} else {                            /* ST_BWD, bwt.c:331-343 */
+				const bool first = n_curr == 0 && cm == 0;
+				if (o_x2 < (u64)min_intv) {
+					if (first && (m1_n == 0 || i + 1 < last_start)) {
+						if (!cur_short) EMIT(e0, e1, e2, i + 1, pend);
+						++m1_n; last_start = i + 1;
+					}
+				} else if (first || o_x2 != curr_last_x2) {
+					PUSH_CAND((int)pend - i + 1, o_s, o_o, o_x2, pend);
+					curr_last_x2 = o_x2;
+				}
+				if (!cur_short) ++j;
 			}
-			if (!cur_short) ++j;
+			if (!two) break;
+			two = false;
+			{
+				ulonglong2 v;
+				u64 x0, x1, x2;
+				u32 ct2;
+				v.x = (u64)ev2.y << 32 | ev2.x; v.y = (u64)ev2.w << 32 | ev2.z;
+				unpack_ent(v, x0, x1, x2, ct2);
+				if (back) { pend = pend2; touches += 1u + (ct2 >> KTAB_BT_SHIFT); o_s = x0; o_o = x1; }
+				else {
+					if (st != ST_FWD) break;    /* the first result ended the sweep: the longer string is never reached */
+					touches += (u64)ref_touches(ix, ik1, ik2);   /* extending the first result */
+					o_s = x1; o_o = x0;
+				}
+				o_x2 = x2;
+			}
 		}
 	}
 	{
@@ -849,6 +917,13 @@ k_smem_c(DevIndex ix, SeedArgs a)
 		u32 f = __reduce_or_sync(FULL_MASK, overflow);
 		if ((threadIdx.x & 31) == 0 && f) atomicOr(a.flags, f);
 	}
+#ifdef BWAG_K1_CLOCKS
+	for (int w = 0; w < BWAG_K1CLK_LANE_WORDS; ++w) {
+		u64 t = clk[w];
+		for (int d = 16; d; d >>= 1) t += __shfl_xor_sync(FULL_MASK, t, d);
+		if ((threadIdx.x & 31) == 0 && t) atomicAdd(a.k1clk + w, t);
+	}
+#endif
 }
 #endif /* !K1_PACKED8 */
 

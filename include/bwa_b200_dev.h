@@ -377,6 +377,15 @@ void bwag_stats_reset(bwag_ctx_t *ctx);
  * mem_chain_flt, of chain_emit; words 264+c, c = chains per read (0..32, 33: more): reads. */
 #define BWAG_K3CLK_WORDS (4 * 66 + 34)
 int bwag_k3_clocks(uint64_t *out, int reset);
+/* builds with -DBWAG_K1_CLOCKS only (else returns -1): copies the seeding kernel k_smem_c's counters (BWAG_K1CLK_WORDS words) to out,
+ * then clears them if reset.  Summed over lanes: loop iterations (a warp's count times 32), iterations that extended forward by a
+ * table lookup / by Occ blocks, backward a list candidate / a mask candidate, those of them that looked up a pair (forward, backward),
+ * clock64() cycles spent handing a finished read over and fetching the next, reads fetched.  Then the CUDA-event time of K1f
+ * (k_smem_fwd) and of k_smem_c in nanoseconds, and the seeding calls. */
+enum { BWAG_K1CLK_ITERS, BWAG_K1CLK_FWD_TAB, BWAG_K1CLK_FWD_OCC, BWAG_K1CLK_BWD_LIST, BWAG_K1CLK_BWD_MASK, BWAG_K1CLK_PAIR_FWD,
+       BWAG_K1CLK_PAIR_BWD, BWAG_K1CLK_TURN_CYC, BWAG_K1CLK_READS, BWAG_K1CLK_LANE_WORDS,
+       BWAG_K1CLK_K1F_NS = BWAG_K1CLK_LANE_WORDS, BWAG_K1CLK_K1C_NS, BWAG_K1CLK_CALLS, BWAG_K1CLK_WORDS };
+int bwag_k1_clocks(uint64_t *out, int reset);
 
 #ifdef __cplusplus
 }
