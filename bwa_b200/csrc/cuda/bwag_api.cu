@@ -76,6 +76,32 @@ extern "C" size_t bwag_blob_bytes(const bwt_t *bwt, int64_t l_pac)
 	return ALIGN256(sizeof(BlobHeader)) + ALIGN256((size_t)bwt->bwt_size * 4 + 64) + ALIGN256((size_t)bwt->n_sa * 8 + 32) + ALIGN256((size_t)l_pac / 4 + 1 + 64);
 }
 
+/* The Occ/BWT words of an updated .bwt uploaded to d (at least bwt_size * 4 + 64 bytes) and re-packed there, in place, into
+ * 32-byte blocks of 64 symbols (bwag_dev.cuh); sb[s]: the counts before superblock s.  The blob holds this beside the SA and
+ * the pac; `bwa-b200 bwt2sa` needs it alone. */
+int occ_upload(void *d, const bwt_t *bwt, u64 sb[BWAG_MAX_SB][4])
+{
+	if (bwt->seq_len >= (u64)BWAG_MAX_SB << BWAG_SB_SHIFT) return set_err("index too large: %llu BWT symbols", (unsigned long long)bwt->seq_len);
+	memset(sb, 0, sizeof(u64) * BWAG_MAX_SB * 4);
+	for (u64 s = 0; s << BWAG_SB_SHIFT < bwt->seq_len; ++s) {   /* counts before symbol s*2^31 = the count words of that file block */
+		const u64 *cnt = (const u64 *)(bwt->bwt + ((s << BWAG_SB_SHIFT) >> 7) * 16);
+		for (int k = 0; k < 4; ++k) sb[s][k] = cnt[k];
+	}
+	CK(cudaMemset(d, 0, ALIGN256((size_t)bwt->bwt_size * 4 + 64)));
+	CK(cudaMemcpy(d, bwt->bwt, (size_t)bwt->bwt_size * 4, cudaMemcpyHostToDevice));
+	{   /* file layout -> 32-byte blocks, in place (bwag_dev.cuh) */
+		const u64 n_blocks = ((u64)bwt->bwt_size * 4 + 63) / 64;
+		DevIndex tmp;
+		memset(&tmp, 0, sizeof(tmp));
+		for (int s = 0; s < BWAG_MAX_SB; ++s)
+			for (int k = 0; k < 4; ++k) tmp.sb[s][k] = sb[s][k];
+		BWAG_LAUNCH(k_occ_pack, (int)((n_blocks + 255) / 256 < 65535 ? (n_blocks + 255) / 256 : 65535), 256, 0, 0, tmp, (uint4 *)d, n_blocks);
+		CK(cudaGetLastError());
+		CK(cudaDeviceSynchronize());
+	}
+	return 0;
+}
+
 extern "C" int bwag_blob_fill(int device, void *d_blob, const bwt_t *bwt, int64_t l_pac, const uint8_t *pac)
 {
 	BlobHeader h;
@@ -89,29 +115,13 @@ extern "C" int bwag_blob_fill(int device, void *d_blob, const bwt_t *bwt, int64_
 		if ((1 << s) != bwt->sa_intv) return set_err("suffix-array interval %d is not a power of two", bwt->sa_intv);
 		h.sa_shift = (u64)s;
 	}
-	if (bwt->seq_len >= (u64)BWAG_MAX_SB << BWAG_SB_SHIFT) return set_err("index too large: %llu BWT symbols", (unsigned long long)bwt->seq_len);
-	for (u64 s = 0; s << BWAG_SB_SHIFT < bwt->seq_len; ++s) {   /* counts before symbol s*2^31 = the count words of that file block */
-		const u64 *cnt = (const u64 *)(bwt->bwt + ((s << BWAG_SB_SHIFT) >> 7) * 16);
-		for (int k = 0; k < 4; ++k) h.sb[s][k] = cnt[k];
-	}
 	h.off_bwt = ALIGN256(sizeof(BlobHeader));
 	h.off_sa = h.off_bwt + ALIGN256((size_t)bwt->bwt_size * 4 + 64);
 	h.off_pac = h.off_sa + ALIGN256((size_t)bwt->n_sa * 8 + 32);
 	h.total = h.off_pac + ALIGN256((size_t)l_pac / 4 + 1 + 64);
 	char *d = (char *)d_blob;
+	if (occ_upload(d + h.off_bwt, bwt, h.sb)) return 1;
 	CK(cudaMemcpy(d, &h, sizeof(h), cudaMemcpyHostToDevice));
-	CK(cudaMemset(d + h.off_bwt, 0, ALIGN256((size_t)bwt->bwt_size * 4 + 64)));
-	CK(cudaMemcpy(d + h.off_bwt, bwt->bwt, (size_t)bwt->bwt_size * 4, cudaMemcpyHostToDevice));
-	{   /* file layout -> 32-byte blocks, in place (bwag_dev.cuh) */
-		const u64 n_blocks = ((u64)bwt->bwt_size * 4 + 63) / 64;
-		DevIndex tmp;
-		memset(&tmp, 0, sizeof(tmp));
-		for (int s = 0; s < BWAG_MAX_SB; ++s)
-			for (int k = 0; k < 4; ++k) tmp.sb[s][k] = h.sb[s][k];
-		BWAG_LAUNCH(k_occ_pack, (int)((n_blocks + 255) / 256 < 65535 ? (n_blocks + 255) / 256 : 65535), 256, 0, 0, tmp, (uint4 *)(d + h.off_bwt), n_blocks);
-		CK(cudaGetLastError());
-		CK(cudaDeviceSynchronize());
-	}
 	CK(cudaMemcpy(d + h.off_sa, bwt->sa, (size_t)bwt->n_sa * 8, cudaMemcpyHostToDevice));
 	CK(cudaMemcpy(d + h.off_pac, pac, (size_t)l_pac / 4 + 1, cudaMemcpyHostToDevice));
 	return 0;

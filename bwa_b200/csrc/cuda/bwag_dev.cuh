@@ -108,6 +108,19 @@ __device__ __forceinline__ int bwag_block_symbol_rank(const DevIndex &ix, const 
 	return c;
 }
 
+/* one LF step: row of the preceding text position (bwt.c:53-59 with bwt_occ bwt.c:107-129) */
+__device__ __forceinline__ u64 lf_step(const DevIndex &ix, u64 k)
+{
+	if (k == ix.primary) return 0;
+	u64 kp = k - (k > ix.primary);                 /* row in the '$'-less BWT == what bwt_occ uses since k != primary */
+	const uint4 *blk = ix.bwt + ((kp >> 6) << 1);    /* one 32-byte sector: counts + bit planes of the 64 symbols around kp */
+	u64 rank;
+	uint4 cn, pl;
+	bwag_ld_block(blk, cn, pl);
+	const int c = bwag_block_symbol_rank(ix, cn, pl, kp, &rank);
+	return ix.L2[c] + rank;
+}
+
 __device__ __forceinline__ int bwag_pac_base(const uint8_t *pac, i64 k) { return pac[k >> 2] >> ((~k & 3) << 1) & 3; }
 
 /* base at position p of the doubled (forward + reverse-complement) coordinate system */

@@ -160,6 +160,7 @@ cudaError_t stream_wait(Lane *c);
 double elapsed_at(Lane *c, const char *stage, const char *file, int line);   /* ms from ev0 to ev1 */
 int fm_grid(const bwag_ctx_t *c, i64 n_items);   /* blocks of 128 for one lane per item, at most 16 per SM */
 int run_sa(bwag_batch_t *b, i64 *rows, i64 n);
+int occ_upload(void *d, const bwt_t *bwt, u64 sb[BWAG_MAX_SB][4]);   /* a .bwt's words, re-packed into 32-byte blocks on the device */
 #define H2D(c, dst, src, bytes) do { CK(cudaMemcpyAsync((dst), (src), (bytes), cudaMemcpyHostToDevice, (c)->stream)); (c)->st.h2d_bytes += (u64)(bytes); } while (0)
 #define D2H(c, dst, src, bytes) do { CK(cudaMemcpyAsync((dst), (src), (bytes), cudaMemcpyDeviceToHost, (c)->stream)); (c)->st.d2h_bytes += (u64)(bytes); } while (0)
 

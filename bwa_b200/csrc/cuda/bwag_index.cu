@@ -14,7 +14,11 @@
  *   4. k_ix_emit writes the group's BWT symbols T[pos-1] and its SA samples (every 32nd row) in place, and records primary.
  * Then the Occ checkpoints every 128 symbols are counted, scanned and interleaved with the symbols (bwt_bwtupdate_core,
  * bwtindex.c:150-172).  Device memory: the packed text (n/4 bytes), one byte per BWT row, the SA sample (n/4 bytes) and one
- * group's working set; nothing of 8 bytes per suffix over the whole text. */
+ * group's working set; nothing of 8 bytes per suffix over the whole text.
+ *
+ * The same group loop (ix_sort) serves `bwa-b200 pac2bwt`, which sorts a .pac text as it is (k_ix_pack_text) and returns the
+ * raw '$'-less BWT of bwt_pac2bwt (k_bw_raw, bwtindex.c:83-145).  `bwa-b200 bwtupdate` adds the Occ checkpoints to such a raw
+ * BWT: counts per block straight from the packed words (k_bw_count), scanned, then interleaved (k_bw_write). */
 #include "bwag_drv.h"
 
 #define IX_HIST_BASES 6          /* buckets of the planning histogram: 4^6, 16 KB of shared counters */
@@ -279,6 +283,63 @@ __global__ void k_occ_write(const uint8_t *B, u64 n, u64 primary, const u64 *occ
 	}
 }
 
+/* T word w = bases 16w..16w+15 of a .pac text taken as it is (pac2bwt), zero beyond n */
+__global__ void k_ix_pack_text(const uint8_t *pac, u64 n, u32 *W, u64 nw)
+{
+	for (u64 w = (u64)blockIdx.x * blockDim.x + threadIdx.x; w < nw; w += (u64)gridDim.x * blockDim.x) {
+		u32 v = 0;
+		for (int j = 0; j < 16; ++j) {
+			const u64 q = (w << 4) + j;
+			if (q < n) v |= (u32)bwag_pac_base(pac, (i64)q) << ((15 - j) << 1);
+		}
+		W[w] = v;
+	}
+}
+
+/* the raw .bwt body of pac2bwt: the '$'-less BWT (symbol j = row j, or j+1 from primary on), 16 symbols per word, first in the
+ * top bits, zero beyond n (bwt_pac2bwt, bwtindex.c:138-140) */
+__global__ void k_bw_raw(const uint8_t *B, u64 n, u64 primary, u32 *out, u64 nw)
+{
+	for (u64 w = (u64)blockIdx.x * blockDim.x + threadIdx.x; w < nw; w += (u64)gridDim.x * blockDim.x) {
+		u32 v = 0;
+		for (int s = 0; s < 16; ++s) {
+			const u64 j = (w << 4) + s;
+			if (j < n) v |= (u32)B[j + (j >= primary)] << ((15 - s) << 1);
+		}
+		out[w] = v;
+	}
+}
+
+/* symbols of each kind in each 128-symbol block of packed words (16 symbols per word, first in the top bits; symbols from n on
+ * are not counted): per word, popcounts of the high bits, the low bits and both */
+__global__ void k_bw_count(const u32 *words, u64 n, u64 *cnt, u64 n_blk)
+{
+	for (u64 b = (u64)blockIdx.x * blockDim.x + threadIdx.x; b < n_blk; b += (u64)gridDim.x * blockDim.x) {
+		u32 c[4] = { 0, 0, 0, 0 };
+		for (int w = 0; w < 8 && b * 128 + (u64)w * 16 < n; ++w) {
+			const u64 left = n - (b * 128 + (u64)w * 16);
+			const int m = left < 16 ? (int)left : 16;
+			const u32 v = words[b * 8 + w] & (m == 16 ? 0xffffffffu : ~(0xffffffffu >> (2 * m)));
+			const u32 nH = __popc(v & 0xaaaaaaaau), nL = __popc(v & 0x55555555u), nT = __popc(v >> 1 & v & 0x55555555u);
+			c[0] += m + nT - nH - nL; c[1] += nL - nT; c[2] += nH - nT; c[3] += nT;
+		}
+		for (int k = 0; k < 4; ++k) cnt[(u64)k * (n_blk + 1) + b] = c[k];
+	}
+}
+
+/* the updated .bwt body from the raw words: k_occ_write's layout (bwt_bwtupdate_core, bwtindex.c:150-172), the words copied */
+__global__ void k_bw_write(const u32 *words, u64 n, const u64 *occ, u64 n_blk, u32 *out)
+{
+	for (u64 b = (u64)blockIdx.x * blockDim.x + threadIdx.x; b < n_blk; b += (u64)gridDim.x * blockDim.x) {
+		u32 *o = out + b * 16;
+		for (int k = 0; k < 4; ++k) { const u64 v = occ[(u64)k * (n_blk + 1) + b]; o[2 * k] = (u32)v; o[2 * k + 1] = (u32)(v >> 32); }
+		int w;
+		for (w = 0; w < 8 && b * 128 + (u64)w * 16 < n; ++w) o[8 + w] = words[b * 8 + w];
+		if (b == n_blk - 1)
+			for (int k = 0; k < 4; ++k) { const u64 v = occ[(u64)k * (n_blk + 1) + n_blk]; o[8 + w + 2 * k] = (u32)v; o[8 + w + 2 * k + 1] = (u32)(v >> 32); }
+	}
+}
+
 /* ------------------------------------------------------------------------------------------------ host driver */
 
 static size_t g_ix_cur, g_ix_peak;
@@ -318,57 +379,49 @@ extern "C" void bwag_built_index_free(bwag_built_index_t *x)
 	x->bwt = 0; x->sa = 0;
 }
 
-extern "C" int bwag_index_build(int device, const uint8_t *pac, int64_t l_pac, bwag_built_index_t *out)
+
+/* BWA_B200_INDEX_BUCKET_BASES: the bucket depth of the planning histogram, forced (tests) */
+static int ix_bucket_bases(int *kb, int *forced)
 {
-	int rc = 0, n_sm = 2, kb = IX_HIST_BASES, forced = 0;
-	const u64 n = 2 * (u64)l_pac, nw = (n + 15) / 16 + 4, n_sa = (n + IX_SA_INTV) / IX_SA_INTV;
-	const u64 n_blk = (n + 127) / 128, bwt_words = (n + 15) / 16 + (n_blk + 1) * 8;
-	u32 *W = 0, *obwt = 0;
-	uint8_t *dpac = 0, *B = 0;
-	u64 *SA = 0, *dcnt = 0, *occ = 0, *hist = 0, *keys0 = 0, *keys1 = 0, *pos0 = 0, *pos1 = 0, *bh = 0, *run_start = 0, *run_len = 0, *run_off = 0, *e_slot = 0;
-	u32 *e_run = 0;
-	u64 cap = 0, h_hist[1 << (2 * IX_HIST_BASES)], h_cnt[4], primary = 0, row = 1, max_group = 0, nblk_cap = 0;
-	size_t free_b = 0, total_b = 0;
-	const char *env = getenv("BWA_B200_INDEX_BUCKET_BASES"), *genv = getenv("BWA_B200_INDEX_GROUP_SUFFIXES");
-	g_ix_cur = g_ix_peak = 0;
-	memset(out, 0, sizeof(*out));
-	if (l_pac <= 0) return set_err("empty reference");
-	if (n >= (u64)BWAG_MAX_SB << BWAG_SB_SHIFT) return set_err("reference too large: %llu bases", (unsigned long long)l_pac);
+	const char *env = getenv("BWA_B200_INDEX_BUCKET_BASES");
+	*kb = IX_HIST_BASES; *forced = 0;
 	if (env && *env) {
-		kb = atoi(env); forced = 1;
-		if (kb < 1 || kb > IX_HIST_BASES) return set_err("BWA_B200_INDEX_BUCKET_BASES must lie in 1..%d", IX_HIST_BASES);
+		*kb = atoi(env); *forced = 1;
+		if (*kb < 1 || *kb > IX_HIST_BASES) return set_err("BWA_B200_INDEX_BUCKET_BASES must lie in 1..%d", IX_HIST_BASES);
 	}
-	{
-		int ndev = 0;
-		if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return set_err("no CUDA device is visible: this library has no CPU path");
-	}
-	if (device < 0) IXCK(cudaGetDevice(&device));
-	IXCK(cudaSetDevice(device));
+	return 0;
+}
+
+/* the device that runs a build, made current; its SM count */
+static int ix_device(int device, int *n_sm)
+{
+	int ndev = 0;
+	*n_sm = 2;
+	if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return set_err("no CUDA device is visible: this library has no CPU path");
+	if (device < 0) CK(cudaGetDevice(&device));
+	CK(cudaSetDevice(device));
 #ifndef BWAG_CUSIM
 	{
 		cudaDeviceProp prop;
-		IXCK(cudaGetDeviceProperties(&prop, device));
-		n_sm = prop.multiProcessorCount;
+		CK(cudaGetDeviceProperties(&prop, device));
+		*n_sm = prop.multiProcessorCount;
 	}
 #endif
-	/* the parts that live through the whole build must fit with room for at least a small group */
-	IXCK(cudaMemGetInfo(&free_b, &total_b));
-	{
-		const double fixed = (double)nw * 4 + (double)(n + 1) + (double)n_sa * 8 + (double)(l_pac / 4 + 1);
-		if (fixed + (double)(64u << 20) > 0.9 * (double)free_b)
-			return set_err("not enough free device memory: the text, BWT and SA sample of %llu bases need %.2f GB, %.2f GB are free",
-			              (unsigned long long)n, fixed / 1e9, (double)free_b / 1e9);
-	}
-	IXCK(ix_malloc((void **)&W, nw * 4));
-	IXCK(cudaMemset(W, 0, nw * 4));
-	IXCK(ix_malloc((void **)&dpac, (size_t)l_pac / 4 + 1));
-	IXCK(cudaMemcpy(dpac, pac, (size_t)l_pac / 4 + 1, cudaMemcpyHostToDevice));
-	BWAG_LAUNCH(k_ix_pack, ix_grid(nw - 4, n_sm), IX_THREADS, 0, 0, dpac, (i64)l_pac, n, W, nw - 4);
-	IXCK(cudaGetLastError());
-	IXCK(cudaDeviceSynchronize());
-	ix_free(dpac, (size_t)l_pac / 4 + 1); dpac = 0;
-	IXCK(ix_malloc((void **)&B, n + 1));
-	IXCK(ix_malloc((void **)&SA, n_sa * 8));
+	return 0;
+}
+
+/* The group loop: sorts the n + 1 suffixes of the packed text W (n bases, zero words beyond it) and writes each row's BWT symbol
+ * to B[row] (B[primary] = 0), every IX_SA_INTV-th row's suffix-array value to SA and the row of suffix 0 to *primary.  Holds
+ * the working set of one group of buckets at a time. */
+static int ix_sort(const u32 *W, u64 n, int n_sm, int kb, int forced, uint8_t *B, u64 *SA, u64 *primary, u64 *n_groups, u64 *max_group_out)
+{
+	int rc = 0;
+	u64 *dcnt = 0, *hist = 0, *keys0 = 0, *keys1 = 0, *pos0 = 0, *pos1 = 0, *bh = 0, *run_start = 0, *run_len = 0, *run_off = 0, *e_slot = 0;
+	u32 *e_run = 0;
+	u64 cap = 0, h_hist[1 << (2 * IX_HIST_BASES)], h_cnt[4], row = 1, max_group = 0, nblk_cap = 0;
+	size_t free_b = 0, total_b = 0;
+	const char *genv = getenv("BWA_B200_INDEX_GROUP_SUFFIXES");
+	*n_groups = 0;
 	IXCK(ix_malloc((void **)&dcnt, 4 * 8));
 	IXCK(cudaMemset(dcnt, 0, 4 * 8));
 
@@ -422,7 +475,7 @@ extern "C" int bwag_index_build(int device, const uint8_t *pac, int64_t l_pac, b
 		u64 m = 0;
 		while (hi < nbk && (hi == lo || (!forced && m + h_hist[hi] <= cap))) m += h_hist[hi++];
 		if (m == 0) { lo = hi; continue; }
-		++out->n_groups;
+		++*n_groups;
 		/* 1. list */
 		IXCK(cudaMemset(dcnt, 0, 3 * 8));   /* dcnt[3] holds primary */
 		BWAG_LAUNCH(k_ix_list, ix_grid(n, n_sm), IX_THREADS, 0, 0, W, n, kb, lo, hi, keys0, pos0, dcnt);
@@ -470,11 +523,52 @@ extern "C" int bwag_index_build(int device, const uint8_t *pac, int64_t l_pac, b
 		lo = hi;
 	}
 	if (row != n + 1) { rc = set_err("sorted %llu rows, expected %llu", (unsigned long long)row, (unsigned long long)n + 1); goto done; }
-	IXCK(cudaMemcpy(&primary, dcnt + 3, 8, cudaMemcpyDeviceToHost));
+	IXCK(cudaMemcpy(primary, dcnt + 3, 8, cudaMemcpyDeviceToHost));
+	*max_group_out = max_group;
+done:
+	ix_free(dcnt, 32); ix_free(hist, ((u64)1 << (2 * kb)) * 8);
 	ix_free(keys0, max_group * 8); ix_free(keys1, max_group * 8); ix_free(pos0, max_group * 8); ix_free(pos1, max_group * 8);
 	ix_free(bh, nblk_cap * 256 * 8); ix_free(run_start, max_group / 2 * 8); ix_free(run_len, max_group / 2 * 8); ix_free(run_off, max_group / 2 * 8);
 	ix_free(e_slot, max_group * 8); ix_free(e_run, max_group * 4);
-	keys0 = keys1 = pos0 = pos1 = bh = run_start = run_len = run_off = e_slot = 0; e_run = 0;
+	return rc;
+}
+
+/* the parts that live through the whole sort must fit with room for at least a small group */
+static int ix_fixed_fits(u64 n, u64 nw, u64 n_sa, u64 pac_bytes)
+{
+	size_t free_b = 0, total_b = 0;
+	CK(cudaMemGetInfo(&free_b, &total_b));
+	const double fixed = (double)nw * 4 + (double)(n + 1) + (double)n_sa * 8 + (double)pac_bytes;
+	if (fixed + (double)(64u << 20) > 0.9 * (double)free_b)
+		return set_err("not enough free device memory: the text, BWT and SA sample of %llu bases need %.2f GB, %.2f GB are free",
+		               (unsigned long long)n, fixed / 1e9, (double)free_b / 1e9);
+	return 0;
+}
+
+extern "C" int bwag_index_build(int device, const uint8_t *pac, int64_t l_pac, bwag_built_index_t *out)
+{
+	int rc = 0, n_sm = 2, kb = IX_HIST_BASES, forced = 0;
+	const u64 n = 2 * (u64)l_pac, nw = (n + 15) / 16 + 4, n_sa = (n + IX_SA_INTV) / IX_SA_INTV;
+	const u64 n_blk = (n + 127) / 128, bwt_words = (n + 15) / 16 + (n_blk + 1) * 8;
+	u32 *W = 0, *obwt = 0;
+	uint8_t *dpac = 0, *B = 0;
+	u64 *SA = 0, *occ = 0, h_cnt[4], primary = 0;
+	g_ix_cur = g_ix_peak = 0;
+	memset(out, 0, sizeof(*out));
+	if (l_pac <= 0) return set_err("empty reference");
+	if (n >= (u64)BWAG_MAX_SB << BWAG_SB_SHIFT) return set_err("reference too large: %llu bases", (unsigned long long)l_pac);
+	if (ix_bucket_bases(&kb, &forced) || ix_device(device, &n_sm) || ix_fixed_fits(n, nw, n_sa, (u64)l_pac / 4 + 1)) return 1;
+	IXCK(ix_malloc((void **)&W, nw * 4));
+	IXCK(cudaMemset(W, 0, nw * 4));
+	IXCK(ix_malloc((void **)&dpac, (size_t)l_pac / 4 + 1));
+	IXCK(cudaMemcpy(dpac, pac, (size_t)l_pac / 4 + 1, cudaMemcpyHostToDevice));
+	BWAG_LAUNCH(k_ix_pack, ix_grid(nw - 4, n_sm), IX_THREADS, 0, 0, dpac, (i64)l_pac, n, W, nw - 4);
+	IXCK(cudaGetLastError());
+	IXCK(cudaDeviceSynchronize());
+	ix_free(dpac, (size_t)l_pac / 4 + 1); dpac = 0;
+	IXCK(ix_malloc((void **)&B, n + 1));
+	IXCK(ix_malloc((void **)&SA, n_sa * 8));
+	if ((rc = ix_sort(W, n, n_sm, kb, forced, B, SA, &primary, (u64 *)&out->n_groups, (u64 *)&out->max_group)) != 0) goto done;
 	ix_free(W, nw * 4); W = 0;
 
 	/* Occ checkpoints: counts per block, scanned per symbol (entry n_blk = total), interleaved with the symbols */
@@ -492,16 +586,101 @@ extern "C" int bwag_index_build(int device, const uint8_t *pac, int64_t l_pac, b
 	if (!out->bwt || !out->sa) { rc = set_err("out of host memory"); goto done; }
 	IXCK(cudaMemcpy(out->bwt, obwt, bwt_words * 4, cudaMemcpyDeviceToHost));
 	IXCK(cudaMemcpy(out->sa, SA, n_sa * 8, cudaMemcpyDeviceToHost));
-	out->max_group = max_group;
 	out->primary = primary; out->seq_len = n; out->bwt_size = bwt_words; out->n_sa = n_sa;
 	out->L2[0] = 0;
 	for (int k = 0; k < 4; ++k) out->L2[k + 1] = out->L2[k] + h_cnt[k];
 done:
 	out->peak_device_bytes = g_ix_peak;
-	ix_free(W, nw * 4); ix_free(dpac, (size_t)l_pac / 4 + 1); ix_free(B, n + 1); ix_free(SA, n_sa * 8); ix_free(dcnt, 32); ix_free(hist, ((u64)1 << (2 * kb)) * 8);
-	ix_free(keys0, max_group * 8); ix_free(keys1, max_group * 8); ix_free(pos0, max_group * 8); ix_free(pos1, max_group * 8);
-	ix_free(bh, nblk_cap * 256 * 8); ix_free(run_start, max_group / 2 * 8); ix_free(run_len, max_group / 2 * 8); ix_free(run_off, max_group / 2 * 8);
-	ix_free(e_slot, max_group * 8); ix_free(e_run, max_group * 4); ix_free(occ, 4 * (n_blk + 1) * 8); ix_free(obwt, bwt_words * 4);
+	ix_free(W, nw * 4); ix_free(dpac, (size_t)l_pac / 4 + 1); ix_free(B, n + 1); ix_free(SA, n_sa * 8);
+	ix_free(occ, 4 * (n_blk + 1) * 8); ix_free(obwt, bwt_words * 4);
 	if (rc) bwag_built_index_free(out);
+	return rc;
+}
+
+/* symbol totals of n packed symbols (L2[1..4] cumulative), by k_bw_count and a scan; occ: 4 (n_blk + 1) words of scratch */
+static int ix_totals(const u32 *words, u64 n, int n_sm, u64 *occ, u64 n_blk, u64 L2[5])
+{
+	u64 h[4];
+	CK(cudaMemset(occ, 0, 4 * (n_blk + 1) * 8));
+	BWAG_LAUNCH(k_bw_count, ix_grid(n_blk, n_sm), IX_THREADS, 0, 0, words, n, occ, n_blk);
+	CK(cudaGetLastError());
+	for (int k = 0; k < 4; ++k) CK(ix_scan(occ + (u64)k * (n_blk + 1), n_blk + 1));
+	for (int k = 0; k < 4; ++k) CK(cudaMemcpy(&h[k], occ + (u64)k * (n_blk + 1) + n_blk, 8, cudaMemcpyDeviceToHost));
+	L2[0] = 0;
+	for (int k = 0; k < 4; ++k) L2[k + 1] = L2[k] + h[k];
+	return 0;
+}
+
+extern "C" int bwag_pac2bwt(int device, const uint8_t *pac, uint64_t n, bwag_raw_bwt_t *out)
+{
+	int rc = 0, n_sm = 2, kb = IX_HIST_BASES, forced = 0;
+	const u64 nw = (n + 15) / 16 + 4, n_sa = (n + IX_SA_INTV) / IX_SA_INTV, pac_bytes = (n + 3) / 4, n_blk = (n + 127) / 128;
+	u32 *W = 0, *raw = 0;
+	uint8_t *dpac = 0, *B = 0;
+	u64 *SA = 0, *occ = 0, primary = 0, n_groups = 0, max_group = 0;
+	g_ix_cur = g_ix_peak = 0;
+	memset(out, 0, sizeof(*out));
+	if (n == 0) return set_err("empty text");
+	if (n >= (u64)BWAG_MAX_SB << BWAG_SB_SHIFT) return set_err("text too large: %llu bases, this build takes fewer than %llu", (unsigned long long)n, (unsigned long long)BWAG_MAX_SB << BWAG_SB_SHIFT);
+	if (ix_bucket_bases(&kb, &forced) || ix_device(device, &n_sm) || ix_fixed_fits(n, nw, n_sa, pac_bytes + 4 * (n_blk + 1) * 8)) return 1;
+	IXCK(ix_malloc((void **)&W, nw * 4));
+	IXCK(cudaMemset(W, 0, nw * 4));
+	IXCK(ix_malloc((void **)&dpac, pac_bytes));
+	IXCK(cudaMemcpy(dpac, pac, pac_bytes, cudaMemcpyHostToDevice));
+	BWAG_LAUNCH(k_ix_pack_text, ix_grid(nw - 4, n_sm), IX_THREADS, 0, 0, dpac, n, W, nw - 4);
+	IXCK(cudaGetLastError());
+	IXCK(cudaDeviceSynchronize());
+	ix_free(dpac, pac_bytes); dpac = 0;
+	IXCK(ix_malloc((void **)&occ, 4 * (n_blk + 1) * 8));
+	if ((rc = ix_totals(W, n, n_sm, occ, n_blk, (u64 *)out->L2)) != 0) goto done;   /* the BWT holds the text's symbols */
+	ix_free(occ, 4 * (n_blk + 1) * 8); occ = 0;
+	IXCK(ix_malloc((void **)&B, n + 1));
+	IXCK(ix_malloc((void **)&SA, n_sa * 8));
+	if ((rc = ix_sort(W, n, n_sm, kb, forced, B, SA, &primary, &n_groups, &max_group)) != 0) goto done;
+	ix_free(W, nw * 4); W = 0;
+	ix_free(SA, n_sa * 8); SA = 0;
+	IXCK(ix_malloc((void **)&raw, (n + 15) / 16 * 4));
+	BWAG_LAUNCH(k_bw_raw, ix_grid((n + 15) / 16, n_sm), IX_THREADS, 0, 0, B, n, primary, raw, (n + 15) / 16);
+	IXCK(cudaGetLastError());
+	if ((out->bwt = (uint32_t *)malloc((n + 15) / 16 * 4)) == 0) { rc = set_err("out of host memory"); goto done; }
+	IXCK(cudaMemcpy(out->bwt, raw, (n + 15) / 16 * 4, cudaMemcpyDeviceToHost));
+	out->primary = primary; out->seq_len = n; out->bwt_size = (n + 15) / 16;
+done:
+	out->peak_device_bytes = g_ix_peak;
+	ix_free(W, nw * 4); ix_free(dpac, pac_bytes); ix_free(B, n + 1); ix_free(SA, n_sa * 8); ix_free(occ, 4 * (n_blk + 1) * 8); ix_free(raw, (n + 15) / 16 * 4);
+	if (rc) { free(out->bwt); out->bwt = 0; }
+	return rc;
+}
+
+extern "C" int bwag_bwtupdate(int device, const uint32_t *raw, uint64_t n, uint32_t *out, uint64_t *peak_device_bytes)
+{
+	int rc = 0, n_sm = 2;
+	const u64 nw = (n + 15) / 16, n_blk = (n + 127) / 128, out_words = nw + (n_blk + 1) * 8;
+	u32 *dw = 0, *dout = 0;
+	u64 *occ = 0;
+	size_t free_b = 0, total_b = 0;
+	g_ix_cur = g_ix_peak = 0;
+	if (n == 0) return set_err("empty BWT");
+	if (ix_device(device, &n_sm)) return 1;
+	IXCK(cudaMemGetInfo(&free_b, &total_b));
+	{
+		const double need = (double)nw * 4 + (double)(n_blk + 1) * 32 + (double)out_words * 4;
+		if (need + (double)(64u << 20) > 0.9 * (double)free_b)
+			{ rc = set_err("not enough free device memory: the update of %llu symbols needs %.2f GB, %.2f GB are free", (unsigned long long)n, need / 1e9, (double)free_b / 1e9); goto done; }
+	}
+	IXCK(ix_malloc((void **)&dw, nw * 4));
+	IXCK(cudaMemcpy(dw, raw, nw * 4, cudaMemcpyHostToDevice));
+	IXCK(ix_malloc((void **)&occ, 4 * (n_blk + 1) * 8));
+	{
+		u64 L2[5];
+		if ((rc = ix_totals(dw, n, n_sm, occ, n_blk, L2)) != 0) goto done;
+	}
+	IXCK(ix_malloc((void **)&dout, out_words * 4));
+	BWAG_LAUNCH(k_bw_write, ix_grid(n_blk, n_sm), IX_THREADS, 0, 0, dw, n, occ, n_blk, dout);
+	IXCK(cudaGetLastError());
+	IXCK(cudaMemcpy(out, dout, out_words * 4, cudaMemcpyDeviceToHost));
+done:
+	if (peak_device_bytes) *peak_device_bytes = g_ix_peak;
+	ix_free(dw, nw * 4); ix_free(occ, 4 * (n_blk + 1) * 8); ix_free(dout, out_words * 4);
 	return rc;
 }

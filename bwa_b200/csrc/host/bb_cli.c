@@ -438,6 +438,11 @@ int main(int argc, char *argv[])
 	bwa_pg = pg.s;
 	if (argc >= 2 && strcmp(argv[1], "shm") == 0) { free(pg.s); return bb_shm_main(argc - 1, argv + 1); }
 	if (argc >= 2 && strcmp(argv[1], "index") == 0) { free(pg.s); return bb_index_main(argc - 1, argv + 1); }
+	if (argc >= 2 && strcmp(argv[1], "fa2pac") == 0) { free(pg.s); return bb_fa2pac_main(argc - 1, argv + 1); }
+	if (argc >= 2 && strcmp(argv[1], "pac2bwt") == 0) { free(pg.s); return bb_pac2bwt_main(argc - 1, argv + 1); }
+	if (argc >= 2 && strcmp(argv[1], "pac2bwtgen") == 0) { free(pg.s); return bb_pac2bwtgen_main(argc - 1, argv + 1); }
+	if (argc >= 2 && strcmp(argv[1], "bwtupdate") == 0) { free(pg.s); return bb_bwtupdate_main(argc - 1, argv + 1); }
+	if (argc >= 2 && strcmp(argv[1], "bwt2sa") == 0) { free(pg.s); return bb_bwt2sa_main(argc - 1, argv + 1); }
 	if (argc >= 2 && strcmp(argv[1], "fastmap") == 0) { free(pg.s); ret = bb_fastmap_main(argc - 1, argv + 1); fflush(stdout); return ret; }
 	if (argc >= 2 && strcmp(argv[1], "aln") == 0) { free(pg.s); ret = bb_aln_main(argc - 1, argv + 1); fflush(stdout); return ret; }
 	if (argc >= 2 && strcmp(argv[1], "samse") == 0) { ret = bb_samse_main(argc - 1, argv + 1); fflush(stdout); free(pg.s); return ret; }
@@ -452,7 +457,14 @@ int main(int argc, char *argv[])
 		fprintf(stderr, "         bwa-b200 sampe [-a maxins] [-o maxocc] [-n INT] [-N INT] [-c FLOAT] [-f out.sam] [-r RG_line] [-P] [-s] [-A]\n"
 		                "                        <idxbase> <in1.sai> <in2.sai> <in1.fq> <in2.fq>   paired-end SAM from two .sai files\n");
 		fprintf(stderr, "         bwa-b200 pemerge [-mu] [-t INT] [-T INT] [-Q INT] <read1.fq> [read2.fq]   merge overlapping read pairs\n");
-		fprintf(stderr, "         bwa-b200 shm [-d|-l] [idxbase]      keep an index resident on the GPU between runs\n\nThe index is the one `bwa index` writes; `bwa-b200 index` writes the same files.\n\n");
+		fprintf(stderr, "         bwa-b200 shm [-d|-l] [idxbase]      keep an index resident on the GPU between runs\n\n");
+		fprintf(stderr, "The steps of `index` on their own:\n");
+		fprintf(stderr, "         bwa-b200 fa2pac [-f] <in.fasta> [<out.prefix>]   .pac .ann .amb (without -f: with the reverse complement)\n");
+		fprintf(stderr, "         bwa-b200 pac2bwt [-d] <in.pac> <out.bwt>         the BWT of the .pac text, without Occ (-d: ignored)\n");
+		fprintf(stderr, "         bwa-b200 pac2bwtgen <in.pac> <out.bwt>           the same file\n");
+		fprintf(stderr, "         bwa-b200 bwtupdate <the.bwt>                     add the Occ checkpoints, in place\n");
+		fprintf(stderr, "         bwa-b200 bwt2sa [-i 32] <in.bwt> <out.sa>        the suffix array, every INT-th row, from the .bwt alone\n\n");
+		fprintf(stderr, "The index is the one `bwa index` writes; `bwa-b200 index` writes the same files.\n\n");
 		return 1;
 	}
 	ret = main_mem(argc - 1, argv + 1);

@@ -150,6 +150,30 @@ const bb_str_t *bb_fq_qual(const bb_fq_t *f);
 /* ---- `bwa-b200 index` (bb_index_build.c) ---- */
 int bb_index_main(int argc, char *argv[]);
 
+/* ---- the .pac/.ann/.amb of a FASTA file, and whole-file writes (bb_pac.c) ---- */
+typedef struct {
+	int64_t l_pac;
+	uint8_t *pac;
+	size_t m_pac;              /* bytes allocated */
+	BB_VEC(bntann1_t) anns;
+	BB_VEC(bntamb1_t) ambs;
+} bb_packed_t;
+void bb_pack_add(bb_packed_t *P, const bb_str_t *name, const bb_str_t *comment, const bb_str_t *seq);
+void bb_pack_add_revcomp(bb_packed_t *P);
+int bb_pack_dump(const bb_packed_t *P, const char *prefix, const char *where);
+void bb_pack_free(bb_packed_t *P);
+int bb_write_whole(const char *fn, const void *a, size_t bytes, const void *b, size_t b_bytes, const char *where);
+int bb_write_index_file(const char *prefix, const char *ext, const void *a, size_t bytes, const void *b, size_t b_bytes, const char *where);
+
+/* ---- `bwa-b200 fa2pac`, `pac2bwt`, `pac2bwtgen`, `bwtupdate`, `bwt2sa` (bb_index_steps.c) ---- */
+int bb_fa2pac_main(int argc, char *argv[]);
+int bb_pac2bwt_main(int argc, char *argv[]);
+int bb_pac2bwtgen_main(int argc, char *argv[]);
+int bb_bwtupdate_main(int argc, char *argv[]);
+int bb_bwt2sa_main(int argc, char *argv[]);
+/* a .bwt file alone, raw or updated (bb_index.c): primary, L2, seq_len = L2[4], bwt_size and the words; no suffix array */
+bwt_t *bb_bwt_restore(const char *fn);
+
 /* ---- `bwa-b200 fastmap` (bb_fastmap.c) ---- */
 int bb_fastmap_main(int argc, char *argv[]);
 

@@ -66,15 +66,12 @@ static char *infer_prefix(const char *hint)
 	return 0;
 }
 
-static bwt_t *load_bwt(const char *prefix)
+bwt_t *bb_bwt_restore(const char *fn)
 {
-	char *fn = bb_malloc(strlen(prefix) + 8);
 	bwt_t *bwt = bb_calloc(1, sizeof(bwt_t));
 	FILE *fp;
 	long fsz;
-	uint64_t hdr[2];
 	int i, j;
-	sprintf(fn, "%s.bwt", prefix);
 	fp = open_or_die(fn, "rb");
 	fseek(fp, 0, SEEK_END); fsz = ftell(fp); fseek(fp, 0, SEEK_SET);
 	bwt->bwt_size = (uint64_t)(fsz - 40) >> 2;
@@ -91,6 +88,17 @@ static bwt_t *load_bwt(const char *prefix)
 			x |= (uint32_t)(((i & 3) == j) + ((i >> 2 & 3) == j) + ((i >> 4 & 3) == j) + ((i >> 6) == j)) << (j << 3);
 		bwt->cnt_table[i] = x;
 	}
+	return bwt;
+}
+
+static bwt_t *load_bwt(const char *prefix)
+{
+	char *fn = bb_malloc(strlen(prefix) + 8);
+	bwt_t *bwt;
+	FILE *fp;
+	uint64_t hdr[2];
+	sprintf(fn, "%s.bwt", prefix);
+	bwt = bb_bwt_restore(fn);
 	sprintf(fn, "%s.sa", prefix);
 	fp = open_or_die(fn, "rb");
 	read_exact(fp, hdr, 8, fn);

@@ -1,9 +1,7 @@
 /* bb_index_build.c -- `bwa-b200 index`: the five index files of a FASTA reference, byte for byte those of the reference's
  * `bwa index` (bwtindex.c:213-330), with the suffix sorting on the GPU (bwag_index_build, bwag_index.cu).
  *
- *   .pac .ann .amb   packed here as bns_fasta2bntseq(..., for_only=1) + bns_dump do (bntseq.c:65-95, 232-333): records as
- *                    kseq reads them, holes = runs of the same non-ACGT character, those bases drawn by lrand48()&3 after
- *                    srand48(11), "(null)" for an empty comment, .pac padded to l_pac/4+1(+1) bytes with l_pac%4 last
+ *   .pac .ann .amb   packed as bns_fasta2bntseq(..., for_only=1) + bns_dump do (bb_pac.c, shared with `fa2pac`), after srand48(11)
  *   .bwt .sa         from the device, written in the layout of bwt_dump_bwt / bwt_dump_sa (bwt.c:385-407)
  *
  * Before it reports success the command loads the new index onto the device and checks every row of it against the text
@@ -12,102 +10,14 @@
 #include <errno.h>
 #include "bb_host.h"
 
-typedef struct {
-	int64_t l_pac;
-	uint8_t *pac;
-	size_t m_pac;              /* bytes allocated */
-	BB_VEC(bntann1_t) anns;
-	BB_VEC(bntamb1_t) ambs;
-} packed_t;
-
-static void add_record(packed_t *P, const bb_str_t *name, const bb_str_t *comment, const bb_str_t *seq)   /* add1, bntseq.c:232-278 */
-{
-	bntann1_t a;
-	size_t i;
-	int lasts = 0;
-	memset(&a, 0, sizeof(a));
-	a.name = bb_strdup(name->l ? name->s : "");
-	a.anno = bb_strdup(comment->l > 0 ? comment->s : "(null)");
-	a.len = (int32_t)seq->l;
-	a.offset = P->l_pac;
-	if ((size_t)(P->l_pac + seq->l) / 4 + 1 > P->m_pac) {
-		size_t m = P->m_pac ? P->m_pac : 1 << 16;
-		while (m < (size_t)(P->l_pac + seq->l) / 4 + 1) m <<= 1;
-		P->pac = bb_realloc(P->pac, m);
-		memset(P->pac + P->m_pac, 0, m - P->m_pac);
-		P->m_pac = m;
-	}
-	for (i = 0; i < seq->l; ++i) {
-		const int ch = seq->s[i];
-		int c = bb_nt4_table[(unsigned char)ch];
-		if (c >= 4) {
-			if (lasts == ch) ++P->ambs.a[P->ambs.n - 1].len;   /* the same character as the one before: the hole goes on */
-			else {
-				bntamb1_t h;
-				h.offset = a.offset + (int64_t)i; h.len = 1; h.amb = (char)ch;
-				bb_vec_push(P->ambs, h);
-				++a.n_ambs;
-			}
-			c = (int)(lrand48() & 3);
-		}
-		lasts = ch;
-		P->pac[P->l_pac >> 2] |= (uint8_t)(c << ((~P->l_pac & 3) << 1));
-		++P->l_pac;
-	}
-	bb_vec_push(P->anns, a);
-}
-
-static int write_file(const char *prefix, const char *ext, const void *a, size_t bytes, const void *b, size_t b_bytes)
-{
-	char *fn = bb_malloc(strlen(prefix) + 8);
-	FILE *fp;
-	int ok;
-	sprintf(fn, "%s%s", prefix, ext);
-	if ((fp = fopen(fn, "wb")) == 0) { fprintf(stderr, "[E::%s] fail to open '%s' for writing: %s\n", "bwa_index", fn, strerror(errno)); free(fn); return 1; }
-	ok = fwrite(a, 1, bytes, fp) == bytes && (!b_bytes || fwrite(b, 1, b_bytes, fp) == b_bytes);
-	ok = fclose(fp) == 0 && ok;
-	if (!ok) fprintf(stderr, "[E::%s] fail to write '%s'\n", "bwa_index", fn);
-	free(fn);
-	return !ok;
-}
-
-static int dump_bns(const packed_t *P, const char *prefix)   /* .pac (bntseq.c:314-327), .ann and .amb (bns_dump) */
-{
-	bb_str_t s = {0, 0, 0};
-	size_t i, n_pac = (size_t)(P->l_pac >> 2) + ((P->l_pac & 3) ? 1 : 0);
-	uint8_t tail[2] = {0, 0};
-	int rc;
-	tail[P->l_pac % 4 == 0] = (uint8_t)(P->l_pac % 4);
-	rc = write_file(prefix, ".pac", P->pac, n_pac, tail, P->l_pac % 4 == 0 ? 2 : 1);
-	if (rc) return rc;
-	bb_putl(&s, P->l_pac); bb_putc(&s, ' '); bb_putl(&s, (int64_t)P->anns.n); bb_puts(&s, " 11\n");
-	for (i = 0; i < P->anns.n; ++i) {
-		const bntann1_t *a = &P->anns.a[i];
-		bb_puts(&s, "0 "); bb_puts(&s, a->name);
-		if (a->anno[0]) { bb_putc(&s, ' '); bb_puts(&s, a->anno); }
-		bb_putc(&s, '\n');
-		bb_putl(&s, a->offset); bb_putc(&s, ' '); bb_putl(&s, a->len); bb_putc(&s, ' '); bb_putl(&s, a->n_ambs); bb_putc(&s, '\n');
-	}
-	rc = write_file(prefix, ".ann", s.s, s.l, 0, 0);
-	s.l = 0;
-	bb_putl(&s, P->l_pac); bb_putc(&s, ' '); bb_putl(&s, (int64_t)P->anns.n); bb_putc(&s, ' '); bb_putl(&s, (int64_t)P->ambs.n); bb_putc(&s, '\n');
-	for (i = 0; i < P->ambs.n; ++i) {
-		const bntamb1_t *h = &P->ambs.a[i];
-		bb_putl(&s, h->offset); bb_putc(&s, ' '); bb_putl(&s, h->len); bb_putc(&s, ' '); bb_putc(&s, h->amb); bb_putc(&s, '\n');
-	}
-	rc = rc || write_file(prefix, ".amb", s.s, s.l, 0, 0);
-	free(s.s);
-	return rc;
-}
-
 static int dump_bwt_sa(const bwag_built_index_t *x, const char *prefix)   /* bwt_dump_bwt, bwt_dump_sa */
 {
 	uint64_t hdr[7];
 	hdr[0] = x->primary;
 	memcpy(hdr + 1, x->L2 + 1, 4 * sizeof(uint64_t));
 	hdr[5] = 32; hdr[6] = x->seq_len;
-	return write_file(prefix, ".bwt", hdr, 5 * 8, x->bwt, (size_t)x->bwt_size * 4) ||
-	       write_file(prefix, ".sa", hdr, 7 * 8, x->sa + 1, (size_t)(x->n_sa - 1) * 8);
+	return bb_write_index_file(prefix, ".bwt", hdr, 5 * 8, x->bwt, (size_t)x->bwt_size * 4, "bwa_index") ||
+	       bb_write_index_file(prefix, ".sa", hdr, 7 * 8, x->sa + 1, (size_t)(x->n_sa - 1) * 8, "bwa_index");
 }
 
 /* every row of the new index against the text, on the device: BWT/text/SA mismatches and order violations are fatal; pairs of
@@ -154,7 +64,7 @@ int bb_index_main(int argc, char *argv[])
 {
 	int c, is_64 = 0, rc = 0, packed = 0;
 	char *prefix = 0;
-	packed_t P;
+	bb_packed_t P;
 	bb_fq_t *fp;
 	const bb_str_t *name, *comment, *seq;
 	bwag_built_index_t x;
@@ -180,10 +90,10 @@ int bb_index_main(int argc, char *argv[])
 
 	memset(&P, 0, sizeof(P));
 	srand48(11);
-	while (bb_fq_read1(fp, &name, &comment, &seq) >= 0) add_record(&P, name, comment, seq);
+	while (bb_fq_read1(fp, &name, &comment, &seq) >= 0) bb_pack_add(&P, name, comment, seq);
 	bb_fq_close(fp);
 	if (P.l_pac == 0) { fprintf(stderr, "[E::%s] no sequence in '%s'\n", "bwa_index", argv[optind]); rc = 1; goto end; }
-	if (dump_bns(&P, prefix)) { rc = 1; goto end; }
+	if (bb_pack_dump(&P, prefix, "bwa_index")) { rc = 1; goto end; }
 	packed = 1;
 	if (bwa_verbose >= 3) fprintf(stderr, "[M::%s] packed %ld sequences (%lld bp, %ld holes) in %.2f sec\n", "bwa_index", (long)P.anns.n, (long long)P.l_pac, (long)P.ambs.n, bb_realtime() - t0);
 
@@ -212,11 +122,7 @@ end:
 		fprintf(stderr, "[E::%s] index '%s' is incomplete: only .pac .ann .amb were written\n", "bwa_index", prefix);
 		free(fn);
 	}
-	{
-		size_t i;
-		for (i = 0; i < P.anns.n; ++i) { free(P.anns.a[i].name); free(P.anns.a[i].anno); }
-	}
-	bb_vec_free(P.anns); bb_vec_free(P.ambs); free(P.pac);
+	bb_pack_free(&P);
 	free(prefix);
 	return rc ? 1 : 0;
 }

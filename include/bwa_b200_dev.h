@@ -71,6 +71,28 @@ typedef struct {
 int bwag_index_build(int device, const uint8_t *pac, int64_t l_pac, bwag_built_index_t *out);
 void bwag_built_index_free(bwag_built_index_t *x);
 
+/* The steps of `bwa index` as commands of their own (bwtindex.c:64-208).  Each fails (bwag_last_error says why) rather than
+ * oversubscribe the device memory cudaMemGetInfo reports free.
+ * bwag_pac2bwt (`bwa-b200 pac2bwt`, `pac2bwtgen`): the BWT of the seq_len bases of pac (the .pac layout) taken as they are, by the
+ * sorter of bwag_index_build: primary, L2 and the '$'-less BWT, 16 symbols per word (first in the top bits), no Occ checkpoints;
+ * the raw .bwt of bwt_pac2bwt.  out->bwt is malloc'ed; the caller frees it. */
+typedef struct {
+	uint64_t primary, seq_len, L2[5];
+	uint64_t bwt_size;          /* (seq_len + 15) / 16 words */
+	uint32_t *bwt;
+	uint64_t peak_device_bytes;
+} bwag_raw_bwt_t;
+int bwag_pac2bwt(int device, const uint8_t *pac, uint64_t seq_len, bwag_raw_bwt_t *out);
+/* bwag_bwtupdate (`bwa-b200 bwtupdate`): the (seq_len + 15) / 16 raw words with the Occ checkpoints interleaved as
+ * bwt_bwtupdate_core does (bwtindex.c:150-172): (seq_len + 15) / 16 + ((seq_len + 127) / 128 + 1) * 8 words into out */
+int bwag_bwtupdate(int device, const uint32_t *raw, uint64_t seq_len, uint32_t *out, uint64_t *peak_device_bytes);
+/* bwag_bwt2sa (`bwa-b200 bwt2sa`): the suffix array sampled every intv-th row (intv a power of two) from an updated BWT alone
+ * (bwt_cal_sa, bwt.c:62-84): sa[r] = SA[r intv] for r < (seq_len + intv) / intv, sa[0] = seq_len.  Ranks the cycle of the LF
+ * mapping in parallel from rulers every `stride` rows (BWA_B200_BWT2SA_STRIDE forces it); fails if LF is not one cycle of
+ * seq_len + 1 rows, i.e. if bwt is not the BWT of any text. */
+typedef struct { uint64_t stride, n_rulers, peak_device_bytes; } bwag_bwt2sa_stats_t;
+int bwag_bwt2sa(int device, const bwt_t *bwt, int intv, uint64_t *sa, bwag_bwt2sa_stats_t *st);
+
 /* Residency across processes (SURVEY.md 8-f3; the reference's counterpart is `bwa shm`, bwashm.c:16-122, which parks the index
  * in POSIX shared memory so that later `bwa mem` runs skip the load).  Device memory lives and dies with its process, so here a
  * process that keeps the index resident (`bwa-b200 shm idxbase`) EXPORTS it -- CUDA IPC handles of the blob, the dense suffix-array
