@@ -153,6 +153,7 @@ static int pick_grid(bwag_ctx_t *c)
 	CK(cudaFuncSetAttribute(k_extend_lane, cudaFuncAttributeMaxDynamicSharedMemorySize, K4L_SMEM_MAX));
 	CK(cudaFuncSetAttribute(k_global_sm, cudaFuncAttributeMaxDynamicSharedMemorySize, K4_SMEM_MAX));
 	CK(cudaFuncSetAttribute(k_global_sm_fast, cudaFuncAttributeMaxDynamicSharedMemorySize, K4_SMEM_MAX));
+	CK(cudaFuncSetAttribute(k_tail_sam, cudaFuncAttributeMaxDynamicSharedMemorySize, TAIL_SAM_SMEM_MAX));   /* one limit for every batch: lanes launch it concurrently */
 	CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_global, K5_THREADS, 0)); c->grid_k5 = c->n_sm * (nb > 0 ? nb : 1);
 #endif
 	return 0;

@@ -155,6 +155,10 @@ struct TailRegsArgs {
 	u64 *n_dregs, *n_tasks, *max_z; int *max_lq, *max_rl;
 };
 
+#ifndef TAIL_SLOT_MAX
+#define TAIL_SLOT_MAX 512   /* bytes of shared memory per lane of k_tail_sam (at most 64 KB per 128-lane block) */
+#endif
+#define TAIL_SAM_SMEM_MAX (128 * TAIL_SLOT_MAX)
 struct TailSamArgs {
 	int n_reads, pe;
 	mem_opt_t opt;
@@ -168,6 +172,7 @@ struct TailSamArgs {
 	const bwag_gres_t *res; const u32 *cigar; const char *md;
 	const char *rg; int l_rg;
 	bwag_samrec_t *rec; char *text; i64 cap_text; u64 *n_text, *n_complex;
+	int slot;                         /* bytes of shared memory per lane for its record (a multiple of 16) */
 };
 
 /* ---- K6 (bwag_localsw.cu) ---- */

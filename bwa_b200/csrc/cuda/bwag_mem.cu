@@ -852,7 +852,7 @@ extern "C" int bwag_tail_regs(bwag_batch_t *b, const mem_opt_t *opt, const bwag_
 	CK(cudaGetLastError());
 	CK(cudaEventRecord(c->ev1, c->stream));
 	if (fetch_counters(c)) return 1;
-	c->st.ms_tail += elapsed_at(c, "tail", __FILE__, __LINE__); ++c->st.n_launch;
+	c->st.ms_tail += elapsed_at(c, "tail_regs", __FILE__, __LINE__); ++c->st.n_launch;
 	const i64 n_tasks = (i64)c->h_cnt->t_tasks;
 	if (n_tasks > cap || (i64)c->h_cnt->t_dregs > cap) return set_err("stage 4: more regions than seeds?");
 	if (n_tasks >= ((i64)1 << 31)) return set_err("stage 4: too many alignment requests in one batch; use smaller chunks");
@@ -918,16 +918,20 @@ extern "C" int bwag_tail_sam(bwag_batch_t *b, const mem_opt_t *opt, const mem_pe
 	g.n_text = &c->d_cnt->t_text; g.n_complex = &c->d_cnt->t_complex;
 	i64 cap_text = b->total_bases + 176 * (i64)n + 4096;
 	const int n_units = pe ? n >> 1 : n;
+	/* a slot holds SEQ and up to 176 bytes of the rest: the records of reads up to TAIL_SLOT_MAX - 176 - l_rg bases are staged */
+	g.slot = (b->max_len + 176 + g.l_rg + 15) & ~15;
+	if (g.slot > TAIL_SLOT_MAX) g.slot = TAIL_SLOT_MAX;
+	const size_t sam_smem = (size_t)128 * g.slot;   /* <= TAIL_SAM_SMEM_MAX, the kernel's limit set once per context */
 	for (int attempt = 0;; ++attempt) {
 		if (buf_reserve(&b->d_text, (size_t)cap_text)) return 1;
 		g.text = (char *)b->d_text.p; g.cap_text = cap_text;
 		if (reset_counters(c)) return 1;
 		CK(cudaEventRecord(c->ev0, c->stream));
-		BWAG_LAUNCH(k_tail_sam, (n_units + 127) / 128, 128, 0, c->stream, g);
+		BWAG_LAUNCH(k_tail_sam, (n_units + 127) / 128, 128, sam_smem, c->stream, g);
 		CK(cudaGetLastError());
 		CK(cudaEventRecord(c->ev1, c->stream));
 		if (fetch_counters(c)) return 1;
-		c->st.ms_tail += elapsed_at(c, "tail", __FILE__, __LINE__); ++c->st.n_launch;
+		c->st.ms_tail += elapsed_at(c, "tail_sam", __FILE__, __LINE__); ++c->st.n_launch;
 		if ((i64)c->h_cnt->t_text <= cap_text) break;
 		if (attempt >= 2) return set_err("stage 4: the text pool keeps overflowing");
 		cap_text = (i64)c->h_cnt->t_text + 4096;

@@ -146,20 +146,22 @@ __global__ void __launch_bounds__(128) k_tail_regs(TailRegsArgs a)
 {
 	const int unit = blockIdx.x * blockDim.x + threadIdx.x;
 	const int n_units = a.pe ? a.n_reads >> 1 : a.n_reads;
+	const bool active = unit < n_units;   /* the whole warp stays for the per-warp reservations */
+	const int lane = threadIdx.x & 31;
 	int max_lq = 0, max_rl = 0;
 	u64 max_z = 0;
-	if (unit < n_units) {
+	{
 		const mem_opt_t &opt = a.opt;
 		mem_alnreg_t regs[2][TAIL_MAXR];
 		int cnt[2] = {0, 0}, bad[2] = {0, 0};
 		const int n_ends = a.pe ? 2 : 1;
 		for (int e = 0; e < n_ends; ++e) {
 			const int r = a.pe ? (unit << 1 | e) : unit;
-			const int n = a.n_raw[r];
+			const int n = active ? a.n_raw[r] : 0;
 			int flag = 0, m = 0;
 			mem_alnreg_t *v = regs[e];
 			if (n > TAIL_MAXR) flag = BWAG_CX_MANY;
-			else {
+			else if (active) {
 				const bwag_xreg_t *x = a.xregs + a.reg_base[r];
 				const i64 cb = a.chain_beg[r];
 				for (int k = 0; k < n; ++k) {
@@ -173,9 +175,17 @@ __global__ void __launch_bounds__(128) k_tail_regs(TailRegsArgs a)
 				}
 				if (!flag) { m = t_dedup(opt, a.ctg.l_pac, n, v); if (m < 0) { flag = BWAG_CX_PATCH; m = 0; } }
 			}
+			/* one reservation of regions and of requests per warp */
+			const int want = flag ? 0 : m;
+			int incl = want;
+			for (int d = 1; d < 32; d <<= 1) { const int t = __shfl_up_sync(FULL_MASK, incl, d); if (lane >= d) incl += t; }
+			const int wsum = __shfl_sync(FULL_MASK, incl, 31);
+			u64 wb = 0, wt = 0;
+			if (lane == 0 && wsum) { wb = atomicAdd(a.n_dregs, (u64)wsum); wt = atomicAdd(a.n_tasks, (u64)wsum); }
+			wb = __shfl_sync(FULL_MASK, wb, 0); wt = __shfl_sync(FULL_MASK, wt, 0);
+			if (!active) continue;
 			if (!flag) {
-				const i64 base = (i64)atomicAdd(a.n_dregs, (u64)m);
-				const i64 t0 = (i64)atomicAdd(a.n_tasks, (u64)m);
+				const i64 base = (i64)wb + incl - want, t0 = (i64)wt + incl - want;
 				a.dreg_beg[r] = base; a.task_beg[r] = t0; a.dreg_n[r] = m;
 				if (base + m > a.cap_dregs || t0 + m > a.cap_tasks) flag = BWAG_CX_CAP;
 				else for (int k = 0; k < m; ++k) {
@@ -199,7 +209,7 @@ __global__ void __launch_bounds__(128) k_tail_regs(TailRegsArgs a)
 			a.cflag[r] = (uint8_t)flag;
 			cnt[e] = m; bad[e] = flag;
 		}
-		if (a.pe) {   /* mem_pestat's per-pair candidate (bwamem_pair.c:88-101); pairs with a flagged end are filled in by the host path */
+		if (active && a.pe) {   /* mem_pestat's per-pair candidate (bwamem_pair.c:88-101); pairs with a flagged end are filled in by the host path */
 			u64 v = 0;
 			if (!bad[0] && !bad[1] && cnt[0] && cnt[1]) {
 				const mem_alnreg_t *r0 = regs[0], *r1 = regs[1];
@@ -444,17 +454,34 @@ __device__ void t_reg2aln(const TailSamArgs &g, int read, int l_query, const mem
 	a.score = ar->score; a.sub = ar->sub > ar->csub ? ar->sub : ar->csub;
 }
 
-struct TW { char *p; int n; };   /* text writer: p == 0 counts only */
-__device__ __forceinline__ void tw_c(TW &w, char c) { if (w.p) w.p[w.n] = c; ++w.n; }
-__device__ __forceinline__ void tw_s(TW &w, const char *s, int l) { if (w.p) for (int i = 0; i < l; ++i) w.p[w.n + i] = s[i]; w.n += l; }
-__device__ void tw_l(TW &w, i64 v)   /* kputl's digits */
+struct TW { char *p; int n, cap; };   /* text writer: bytes at or beyond cap are counted, not written */
+__device__ __forceinline__ void tw_c(TW &w, char c) { if (w.n < w.cap) w.p[w.n] = c; ++w.n; }
+__device__ __forceinline__ void tw_s(TW &w, const char *s, int l) { const int lim = min(l, w.cap - w.n); for (int i = 0; i < lim; ++i) w.p[w.n + i] = s[i]; w.n += l; }
+__device__ void tw_l(TW &w, i64 v)   /* kputl's digits, last digit first */
 {
-	char buf[24];
-	int n = 0;
 	u64 u = v < 0 ? (u64)(-(v + 1)) + 1u : (u64)v;
-	do { buf[n++] = (char)('0' + u % 10); u /= 10; } while (u);
-	if (v < 0) buf[n++] = '-';
-	while (n) tw_c(w, buf[--n]);
+	int nd = 1;
+	for (u64 t = u; t >= 10; t /= 10) ++nd;
+	if (v < 0) tw_c(w, '-');
+	for (int k = nd - 1; k >= 0; --k, u /= 10) if (w.n + k < w.cap) w.p[w.n + k] = (char)('0' + u % 10);
+	w.n += nd;
+}
+/* SEQ: the read's codes as ACGTN, or reverse-complemented, from aligned 4-byte loads (the batch's code buffer has 16 bytes of
+ * padding past its last read, so the word holding a read's last code never leaves it) */
+__device__ void tw_seq(TW &w, const uint8_t *codes, int l_seq, int rev)
+{
+	const int mis = (int)((size_t)codes & 3), lim = min(l_seq, w.cap - w.n);
+	const u32 *wp = (const u32 *)(codes - mis);
+	const u32 tab = rev ? 0x41434754u : 0x54474341u;   /* "TGCA" / "ACGT", code 0 in the low byte */
+	char *d = w.p + w.n;
+	u32 x = 0;
+	for (int i = 0; i < lim; ++i) {
+		const int j = rev ? l_seq - 1 - i + mis : i + mis;
+		if (i == 0 || (j & 3) == (rev ? 3 : 0)) x = wp[j >> 2];
+		const u32 c = x >> ((j & 3) << 3) & 0xff;
+		d[i] = c < 4 ? (char)(tab >> (c << 3)) : 'N';
+	}
+	w.n += l_seq;
 }
 __device__ void tw_cigar(TW &w, const TAln &al)
 {
@@ -505,12 +532,7 @@ __device__ void t_aln2sam(const TailSamArgs &g, TW &w, const uint8_t *codes, int
 		} else tw_c(w, '0');
 	} else tw_s(w, "*\t0\t0", 5);
 	tw_c(w, '\t');
-	if (w.p) {
-		char *d = w.p + w.n;
-		if (!p.is_rev) for (int i = 0; i < l_seq; ++i) { const int c = codes[i]; d[i] = "ACGTN"[c > 4 ? 4 : c]; }
-		else for (int i = 0; i < l_seq; ++i) { const int c = codes[l_seq - 1 - i]; d[i] = "TGCAN"[c > 4 ? 4 : c]; }
-	}
-	w.n += l_seq;
+	tw_seq(w, codes, l_seq, p.is_rev);
 	tw_c(w, '\t');
 	*len_a = w.n - w0;
 	*qrev = p.is_rev;
@@ -545,12 +567,12 @@ __global__ void __launch_bounds__(128) k_tail_sam(TailSamArgs g)
 {
 	const int unit = blockIdx.x * blockDim.x + threadIdx.x;
 	const int n_units = g.pe ? g.n_reads >> 1 : g.n_reads;
-	if (unit >= n_units) return;
+	const bool active = unit < n_units;   /* the whole warp stays for the records' copy-out */
 	const mem_opt_t &opt = g.opt;
 	const int n_ends = g.pe ? 2 : 1;
 	mem_alnreg_t regs[2][TAIL_MAXR];
 	int n[2] = {0, 0}, len[2] = {0, 0}, rd[2] = {0, 0}, cx = 0;
-	for (int e = 0; e < n_ends; ++e) {
+	for (int e = 0; e < n_ends && active; ++e) {
 		const int r = g.pe ? (unit << 1 | e) : unit;
 		rd[e] = r;
 		len[e] = (int)(g.off[r + 1] - g.off[r]);
@@ -560,7 +582,8 @@ __global__ void __launch_bounds__(128) k_tail_sam(TailSamArgs g)
 	TAln h[2], rec[2];
 	bool have_rec[2] = {false, false};
 	int extra_flag = 1;
-	if (!cx && !g.pe) {   /* worker2, single-end (bwamem.c:1222-1226) */
+	if (!active) {
+	} else if (!cx && !g.pe) {   /* worker2, single-end (bwamem.c:1222-1226) */
 		t_mark_primary(opt, n[0], regs[0], g.n_processed + unit);
 		const int k = t_reg2sam_pick(opt, n[0], regs[0], &cx);
 		if (!cx) t_reg2aln(g, rd[0], len[0], k >= 0 ? &regs[0][k] : 0, &rec[0], &cx);
@@ -654,23 +677,56 @@ __global__ void __launch_bounds__(128) k_tail_sam(TailSamArgs g)
 		}
 		have_rec[0] = have_rec[1] = true;
 	}
-	if (!cx && !g.pe) have_rec[0] = true;
+	if (active && !cx && !g.pe) have_rec[0] = true;
+	/* Each lane formats its record once, into its slot of g.slot bytes of shared memory.  The warp then takes one span of the
+	 * text pool for all records that fitted their slots, each rounded up to 16 bytes, and copies them out with coalesced 16-byte
+	 * stores.  A record longer than its slot (long reads, long contig names or read groups) takes a span of its own and is
+	 * formatted a second time, straight into the pool. */
+#ifdef BWAG_CUSIM
+	char *const wbuf = (char *)cusim_dyn_smem + (size_t)(threadIdx.x & ~31) * g.slot;
+#else
+	extern __shared__ int4 tail_dyn[];
+	char *const wbuf = (char *)tail_dyn + (size_t)(threadIdx.x & ~31) * g.slot;
+#endif
+	const int lane = threadIdx.x & 31;
+	char *const slot = wbuf + lane * g.slot;
 	for (int e = 0; e < n_ends; ++e) {
-		bwag_samrec_t out;
-		out.off = 0; out.len_a = out.len_b = 0; out.flags = 0; out.pad = 0;
-		if (cx || !have_rec[e]) out.flags = BWAG_REC_COMPLEX | (u32)cx << 8;
-		else {
-			const uint8_t *codes = g.codes + g.off[rd[e]];
-			const TAln *mate = g.pe ? &h[!e] : 0;
-			TW w; w.p = 0; w.n = 0;
-			int la = 0, qrev = 0;
-			t_aln2sam(g, w, codes, len[e], rec[e], mate, &la, &qrev);
-			const int total = w.n;
-			const i64 o = (i64)atomicAdd(g.n_text, (u64)((total + 7) & ~7));
-			out.off = o; out.len_a = la; out.len_b = total - la; out.flags = BWAG_REC_TEXT | (qrev ? BWAG_REC_QREV : 0);
-			if (o + total <= g.cap_text) { w.p = g.text + o; w.n = 0; t_aln2sam(g, w, codes, len[e], rec[e], mate, &la, &qrev); }
+		const bool text = active && !cx && have_rec[e];
+		const uint8_t *codes = text ? g.codes + g.off[rd[e]] : 0;
+		const TAln *mate = g.pe ? &h[!e] : 0;
+		int total = 0, la = 0, qrev = 0;
+		if (text) { TW w = { slot, 0, g.slot }; t_aln2sam(g, w, codes, len[e], rec[e], mate, &la, &qrev); total = w.n; }
+		const int span = (total + 15) & ~15, staged = total <= g.slot ? span : 0;
+		int incl = staged;
+		for (int d = 1; d < 32; d <<= 1) { const int v = __shfl_up_sync(FULL_MASK, incl, d); if (lane >= d) incl += v; }
+		const int wsum = __shfl_sync(FULL_MASK, incl, 31);
+		u64 base = 0;
+		if (lane == 0 && wsum) base = atomicAdd(g.n_text, (u64)wsum);
+		base = __shfl_sync(FULL_MASK, base, 0);
+		i64 o = (i64)base + incl - staged;
+		if (!staged && total) {
+			o = (i64)atomicAdd(g.n_text, (u64)span);
+			if (o + span <= g.cap_text) { TW w = { g.text + o, 0, span }; t_aln2sam(g, w, codes, len[e], rec[e], mate, &la, &qrev); }
 		}
-		g.rec[rd[e]] = out;
+		__syncwarp();
+		if ((i64)base + wsum <= g.cap_text) {   /* else the pool overflows: the launch is repeated with room for n_text */
+			for (u32 m = __ballot_sync(FULL_MASK, staged > 0); m; m &= m - 1) {
+				const int j = __ffs(m) - 1, nv = __shfl_sync(FULL_MASK, staged, j) >> 4;
+				const i64 oj = __shfl_sync(FULL_MASK, o, j);
+				const int4 *src = (const int4 *)(wbuf + j * g.slot);
+				int4 *dst = (int4 *)(g.text + oj);
+				for (int k = lane; k < nv; k += 32) dst[k] = src[k];
+			}
+		}
+		__syncwarp();
+		if (active) {
+			bwag_samrec_t out;
+			out.off = 0; out.len_a = out.len_b = 0; out.flags = 0; out.pad = 0;
+			if (!text) out.flags = BWAG_REC_COMPLEX | (u32)cx << 8;
+			else { out.off = o; out.len_a = la; out.len_b = total - la; out.flags = BWAG_REC_TEXT | (qrev ? BWAG_REC_QREV : 0); }
+			g.rec[rd[e]] = out;
+		}
 	}
-	if (cx) atomicAdd(g.n_complex, (u64)n_ends);
+	const int n_cx = __reduce_add_sync(FULL_MASK, active && cx ? n_ends : 0);
+	if (lane == 0 && n_cx) atomicAdd(g.n_complex, (u64)n_cx);
 }
