@@ -47,16 +47,16 @@ oracle:
 
 # ---- test-only artefacts ----
 testbin: tests/_build/bwa-b200-oracle
-tests/_build/bwa-b200-oracle: $(HOST_OBJ) build/host/bb_main.o oracle/oracle_fm.c oracle/oracle_sw.c oracle/oracle_stages.c tests/oracle_index.c tests/oracle_index_steps.c tests/oracle_fastmap.c tests/oracle_aln.c tests/oracle_samse.c tests/oracle_sampe.c tests/oracle_pemerge.c
+tests/_build/bwa-b200-oracle: $(HOST_OBJ) build/host/bb_main.o oracle/oracle_fm.c oracle/oracle_sw.c oracle/oracle_stages.c tests/oracle_index.c tests/oracle_index_steps.c tests/oracle_maxk.c tests/oracle_fastmap.c tests/oracle_aln.c tests/oracle_samse.c tests/oracle_sampe.c tests/oracle_pemerge.c
 	@mkdir -p tests/_build
-	$(CC) $(CFLAGS) -O3 -Ioracle -o $@ build/host/bb_main.o $(HOST_OBJ) oracle/oracle_fm.c oracle/oracle_sw.c oracle/oracle_stages.c tests/oracle_index.c tests/oracle_index_steps.c tests/oracle_fastmap.c tests/oracle_aln.c tests/oracle_samse.c tests/oracle_sampe.c tests/oracle_pemerge.c -lz -lm -lpthread
+	$(CC) $(CFLAGS) -O3 -Ioracle -o $@ build/host/bb_main.o $(HOST_OBJ) oracle/oracle_fm.c oracle/oracle_sw.c oracle/oracle_stages.c tests/oracle_index.c tests/oracle_index_steps.c tests/oracle_maxk.c tests/oracle_fastmap.c tests/oracle_aln.c tests/oracle_samse.c tests/oracle_sampe.c tests/oracle_pemerge.c -lz -lm -lpthread
 
 # host pipeline under ThreadSanitizer over the CPU oracle stages (TEST ONLY): make tsan
 TSAN_CC ?= $(shell test -x /usr/bin/gcc && echo /usr/bin/gcc || echo $(CC))   # a compiler whose installation ships libtsan
 tsan: tests/_build/bwa-b200-tsan
-tests/_build/bwa-b200-tsan: $(HOST_SRC) $(HOST)/bb_cli.c $(wildcard $(HOST)/*.h) $(wildcard include/*.h) oracle/oracle_fm.c oracle/oracle_sw.c oracle/oracle_stages.c tests/oracle_index.c tests/oracle_index_steps.c tests/oracle_fastmap.c tests/oracle_aln.c tests/oracle_samse.c tests/oracle_sampe.c tests/oracle_pemerge.c
+tests/_build/bwa-b200-tsan: $(HOST_SRC) $(HOST)/bb_cli.c $(wildcard $(HOST)/*.h) $(wildcard include/*.h) oracle/oracle_fm.c oracle/oracle_sw.c oracle/oracle_stages.c tests/oracle_index.c tests/oracle_index_steps.c tests/oracle_maxk.c tests/oracle_fastmap.c tests/oracle_aln.c tests/oracle_samse.c tests/oracle_sampe.c tests/oracle_pemerge.c
 	@mkdir -p tests/_build
-	$(TSAN_CC) -fsanitize=thread -O1 -g -Wall -Wno-unused-function -Iinclude -I$(HOST) -Ioracle -pthread -DBB_MAIN -o $@ $(HOST_SRC) $(HOST)/bb_cli.c oracle/oracle_fm.c oracle/oracle_sw.c oracle/oracle_stages.c tests/oracle_index.c tests/oracle_index_steps.c tests/oracle_fastmap.c tests/oracle_aln.c tests/oracle_samse.c tests/oracle_sampe.c tests/oracle_pemerge.c -lz -lm -lpthread
+	$(TSAN_CC) -fsanitize=thread -O1 -g -Wall -Wno-unused-function -Iinclude -I$(HOST) -Ioracle -pthread -DBB_MAIN -o $@ $(HOST_SRC) $(HOST)/bb_cli.c oracle/oracle_fm.c oracle/oracle_sw.c oracle/oracle_stages.c tests/oracle_index.c tests/oracle_index_steps.c tests/oracle_maxk.c tests/oracle_fastmap.c tests/oracle_aln.c tests/oracle_samse.c tests/oracle_sampe.c tests/oracle_pemerge.c -lz -lm -lpthread
 
 clean:
 	rm -rf build bwa_b200/libbwa_b200.so bwa_b200/bwa-b200 tests/_build

@@ -146,6 +146,9 @@ struct bwag_batch {
 	/* pemerge (bwag_pemerge.cu; K6's buffers hold its tasks, codes and alignments) */
 	DevBuf d_pm_qual, d_pm_hasq, d_pm_names, d_pm_noff, d_pm_q, d_pm_code, d_pm_ovl, d_pm_tlen, d_pm_tbeg, d_pm_text, d_pm_cnt;
 	HostBuf h_pm_text, h_pm_cnt;
+	/* maxk (bwag_maxk.cu) */
+	DevBuf d_mk_woff, d_mk_cnt, d_mk_ctr, d_mk_scratch;
+	HostBuf h_mk_woff, h_mk_ctr;
 	int tail_ready;             /* bwag_tail_regs ran on this batch */
 	int regs_on_device;          /* bwag_chain_extend left the regions in HBM */
 };

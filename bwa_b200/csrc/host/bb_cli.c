@@ -443,6 +443,7 @@ int main(int argc, char *argv[])
 	if (argc >= 2 && strcmp(argv[1], "pac2bwtgen") == 0) { free(pg.s); return bb_pac2bwtgen_main(argc - 1, argv + 1); }
 	if (argc >= 2 && strcmp(argv[1], "bwtupdate") == 0) { free(pg.s); return bb_bwtupdate_main(argc - 1, argv + 1); }
 	if (argc >= 2 && strcmp(argv[1], "bwt2sa") == 0) { free(pg.s); return bb_bwt2sa_main(argc - 1, argv + 1); }
+	if (argc >= 2 && strcmp(argv[1], "maxk") == 0) { free(pg.s); ret = bb_maxk_main(argc - 1, argv + 1); fflush(stdout); return ret; }
 	if (argc >= 2 && strcmp(argv[1], "fastmap") == 0) { free(pg.s); ret = bb_fastmap_main(argc - 1, argv + 1); fflush(stdout); return ret; }
 	if (argc >= 2 && strcmp(argv[1], "aln") == 0) { free(pg.s); ret = bb_aln_main(argc - 1, argv + 1); fflush(stdout); return ret; }
 	if (argc >= 2 && strcmp(argv[1], "samse") == 0) { ret = bb_samse_main(argc - 1, argv + 1); fflush(stdout); free(pg.s); return ret; }
@@ -452,6 +453,7 @@ int main(int argc, char *argv[])
 		fprintf(stderr, "\nProgram: bwa-b200 (BWA-MEM seed-and-extend on NVIDIA H100)\nVersion: %s\n\nUsage:   bwa-b200 index [-p prefix] <in.fasta[.gz]>   build the index files on the GPU\n", BB_VERSION);
 		fprintf(stderr, "         bwa-b200 mem [options] <idxbase> <in1.fq> [in2.fq]\n");
 		fprintf(stderr, "         bwa-b200 fastmap [options] <idxbase> <in.fq>   list each read's SMEMs and their positions\n");
+		fprintf(stderr, "         bwa-b200 maxk [-s] <in.bwt> <seq.fa>            histogram of each base's longest SMEM (-s: against its own index)\n");
 		fprintf(stderr, "         bwa-b200 aln [options] <idxbase> <in.fq>       BWA-backtrack: the .sai file of `bwa aln`\n");
 		fprintf(stderr, "         bwa-b200 samse [-n max_occ] [-f out.sam] [-r RG_line] <idxbase> <in.sai> <in.fq>   single-end SAM from a .sai file\n");
 		fprintf(stderr, "         bwa-b200 sampe [-a maxins] [-o maxocc] [-n INT] [-N INT] [-c FLOAT] [-f out.sam] [-r RG_line] [-P] [-s] [-A]\n"

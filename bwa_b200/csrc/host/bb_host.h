@@ -173,6 +173,12 @@ int bb_bwtupdate_main(int argc, char *argv[]);
 int bb_bwt2sa_main(int argc, char *argv[]);
 /* a .bwt file alone, raw or updated (bb_index.c): primary, L2, seq_len = L2[4], bwt_size and the words; no suffix array */
 bwt_t *bb_bwt_restore(const char *fn);
+/* (bb_index_steps.c) a .bwt file of a non-empty text, raw (updated = 0) or with its Occ checkpoints (updated = 1); NULL after a
+ * message otherwise */
+bwt_t *bb_read_bwt(const char *fn, int updated, const char *where);
+
+/* ---- `bwa-b200 maxk` (bb_maxk.c) ---- */
+int bb_maxk_main(int argc, char *argv[]);
 
 /* ---- `bwa-b200 fastmap` (bb_fastmap.c) ---- */
 int bb_fastmap_main(int argc, char *argv[]);

@@ -127,8 +127,7 @@ int bb_pac2bwtgen_main(int argc, char *argv[])
 static uint64_t raw_words(uint64_t n) { return (n + 15) / 16; }
 static uint64_t updated_words(uint64_t n) { return (n + 15) / 16 + ((n + 127) / 128 + 1) * 8; }
 
-/* a .bwt file of a non-empty text, raw (updated = 0) or with its Occ checkpoints (updated = 1); NULL after a message otherwise */
-static bwt_t *read_bwt(const char *fn, int updated, const char *where)
+bwt_t *bb_read_bwt(const char *fn, int updated, const char *where)
 {
 	int64_t size;
 	bwt_t *bwt;
@@ -157,7 +156,7 @@ int bb_bwtupdate_main(int argc, char *argv[])
 	double t = bb_realtime();
 	int rc;
 	if (argc != 2) { fprintf(stderr, "Usage: bwa-b200 bwtupdate <the.bwt>\n"); return 1; }
-	if ((bwt = read_bwt(argv[1], 0, where)) == 0) return 1;
+	if ((bwt = bb_read_bwt(argv[1], 0, where)) == 0) return 1;
 	out = bb_malloc((size_t)updated_words(bwt->seq_len) * 4);
 	if ((rc = bwag_bwtupdate(-1, bwt->bwt, bwt->seq_len, out, &peak)) != 0) rc = device_failed(rc, where, "Occ builder");
 	else {
@@ -188,7 +187,7 @@ int bb_bwt2sa_main(int argc, char *argv[])
 	}
 	if (optind + 2 > argc) { fprintf(stderr, "Usage: bwa-b200 bwt2sa [-i %d] <in.bwt> <out.sa>\n", intv); return 1; }
 	if (intv < 1 || (intv & (intv - 1))) { fprintf(stderr, "[E::%s] the SA sample interval %d is not a power of two >= 1\n", where, intv); return 1; }
-	if ((bwt = read_bwt(argv[optind], 1, where)) == 0) return 1;
+	if ((bwt = bb_read_bwt(argv[optind], 1, where)) == 0) return 1;
 	n_sa = (bwt->seq_len + (uint64_t)intv) / (uint64_t)intv;
 	sa = malloc((size_t)n_sa * 8);
 	if (!sa) { fprintf(stderr, "[E::%s] out of host memory for %llu suffix-array entries\n", where, (unsigned long long)n_sa); free(bwt->bwt); free(bwt); return 1; }

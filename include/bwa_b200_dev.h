@@ -159,6 +159,24 @@ typedef struct {
 } bwag_fastmap_t;
 int bwag_fastmap(bwag_batch_t *b, const bwag_fastmap_par_t *par, bwag_fastmap_t *out);
 
+/* ---- longest-match histogram of `bwa maxk` (replaces the smem_next loop of main_maxk, maxk.c:34-55) ----------------------------
+ * bwag_ctx_create_occ: a context over an updated .bwt alone (bwt_restore_bwt): the Occ blocks, no suffix array, no text; NULL
+ * (bwag_last_error says why) without a device.  bwag_maxk: per base of each of the batch's sequences, the longest match of the
+ * reference's chain of bwt_smem1a calls (min_intv as given, max_intv 0) that covers it, capped at 255 (0 for N and for bases no
+ * match covers); hist[v] += the number of bases of value v.  window > 0: each sequence is cut into windows of that many bases
+ * that run in parallel, which gives the reference's bytes only when each of the four bases occurs at least min_intv times in the
+ * BWT (L2[c+1] - L2[c] >= min_intv; the caller checks); window <= 0: one window per sequence, the reference's chain as it runs.
+ * BWAG_UNSUPPORTED from the CPU oracle of the tests. */
+typedef struct {
+	int64_t window, n_windows;   /* the window used (whole-sequence windows: the longest sequence) and the batch's windows */
+	int list_cap, n_repeat;      /* interval-list entries per lane, and the runs repeated because a list outgrew them */
+	double ms_kernel, ms_hist;   /* CUDA-event time of the search (all runs) and of the binning */
+	double max_window_ms;        /* the longest time one lane spent on one window (device clock) */
+	uint64_t occ_touches;        /* Occ blocks touched as the reference counts them (bwt.c:194-197) */
+} bwag_maxk_stats_t;
+bwag_ctx_t *bwag_ctx_create_occ(int device, const bwt_t *bwt);
+int bwag_maxk(bwag_batch_t *b, int min_intv, int64_t window, uint64_t hist[256], bwag_maxk_stats_t *st);
+
 /* ---- BWA-backtrack search of `bwa aln` (replaces bwa_cal_sa_reg_gap + bwt_match_gap, bwtaln.c:83-126, bwtgap.c:109-264) -------
  * The batch's codes are the searched bases of each read in input order (after barcode removal and quality trimming).  Per read:
  * the widths of the reversed read (and of its seed), then the bounded-difference backtracking search with the reference's
