@@ -131,8 +131,8 @@ __device__ __forceinline__ int dev_intv2rid(const ChainArgs &a, i64 rb, i64 re) 
 }
 __device__ __forceinline__ int dev_max_gap(const ChainArgs &p, int qlen) /* bwamem.c:647-654 */
 {
-	int l_del = (int)((double)(qlen * p.a - p.o_del) / p.e_del + 1.);
-	int l_ins = (int)((double)(qlen * p.a - p.o_ins) / p.e_ins + 1.);
+	int l_del = bwag_trunc_i32((double)(qlen * p.a - p.o_del) / p.e_del + 1.);
+	int l_ins = bwag_trunc_i32((double)(qlen * p.a - p.o_ins) / p.e_ins + 1.);
 	int l = l_del > l_ins ? l_del : l_ins;
 	l = l > 1 ? l : 1;
 	return l < p.w << 1 ? l : p.w << 1;
@@ -256,7 +256,7 @@ template <class W, class A> __device__ void sort_comb(const W &w, A a, int lo, i
 	const double shrink = 1.2473309501039786540366528676643;
 	int gap = n, moved;
 	do {
-		if (gap > 2) { gap = (int)(gap / shrink); if (gap == 9 || gap == 10) gap = 11; }
+		if (gap > 2) { gap = (int)(gap / shrink); if (gap == 9 || gap == 10) gap = 11; }   /* in range: 0 < gap / shrink < gap */
 		moved = 0;
 		for (int p = lo; p + gap < lo + n; ++p)
 			if (W_LT(a[p + gap], a[p])) { auto t = a[p]; a[p] = a[p + gap]; a[p + gap] = t; moved = 1; }

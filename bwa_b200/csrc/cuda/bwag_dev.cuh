@@ -121,6 +121,15 @@ __device__ __forceinline__ u64 lf_step(const DevIndex &ix, u64 k)
 	return ix.L2[c] + rank;
 }
 
+/* (int)x as the reference's x86-64 build computes it (cvttsd2si): x truncated toward zero when that fits an int, else INT_MIN --
+ * for NaN, +-inf and every out-of-range value alike.  The device's own conversion (cvt.rzi.s32.f64) saturates instead (+inf and
+ * large values give INT_MAX, NaN gives 0), which differs where the reference divides by a gap extension of 0 (-E 0): its band and
+ * gap limits then come out as INT_MIN and are clamped to 1. */
+__device__ __forceinline__ int bwag_trunc_i32(double x)
+{
+	return x > -2147483649.0 && x < 2147483648.0 ? (int)x : (-2147483647 - 1);
+}
+
 __device__ __forceinline__ int bwag_pac_base(const uint8_t *pac, i64 k) { return pac[k >> 2] >> ((~k & 3) << 1) & 3; }
 
 /* base at position p of the doubled (forward + reverse-complement) coordinate system */

@@ -34,8 +34,8 @@ __device__ __forceinline__ int warp_min(int v) { return __reduce_min_sync(FULL_M
 
 __device__ __forceinline__ int dev_cal_max_gap(const bwag_sw_par_t &p, int qlen) /* bwamem.c:647-654 */
 {
-	int l_del = (int)((double)(qlen * p.a - p.o_del) / p.e_del + 1.);
-	int l_ins = (int)((double)(qlen * p.a - p.o_ins) / p.e_ins + 1.);
+	int l_del = bwag_trunc_i32((double)(qlen * p.a - p.o_del) / p.e_del + 1.);
+	int l_ins = bwag_trunc_i32((double)(qlen * p.a - p.o_ins) / p.e_ins + 1.);
 	int l = l_del > l_ins ? l_del : l_ins;
 	l = l > 1 ? l : 1;
 	return l < p.w << 1 ? l : p.w << 1;
@@ -58,9 +58,9 @@ __device__ __forceinline__ int warp_ksw_extend(int lane, int qlen, const uint8_t
 			E[j] = 0;
 		}
 		for (int k = 0; k < 25; ++k) maxsc = maxsc > mat[k] ? maxsc : mat[k];
-		int max_ins = (int)((double)(qlen * maxsc + end_bonus - o_ins) / e_ins + 1.); max_ins = max_ins > 1 ? max_ins : 1;
+		int max_ins = bwag_trunc_i32((double)(qlen * maxsc + end_bonus - o_ins) / e_ins + 1.); max_ins = max_ins > 1 ? max_ins : 1;
 		w = w < max_ins ? w : max_ins;
-		int max_del = (int)((double)(qlen * maxsc + end_bonus - o_del) / e_del + 1.); max_del = max_del > 1 ? max_del : 1;
+		int max_del = bwag_trunc_i32((double)(qlen * maxsc + end_bonus - o_del) / e_del + 1.); max_del = max_del > 1 ? max_del : 1;
 		w = w < max_del ? w : max_del;
 	}
 	__syncwarp();
@@ -186,9 +186,9 @@ __device__ __forceinline__ int warp_ksw_extend_fast(int lane, int qlen, typename
 			A::st_he(he + 8 * j, v > 0 ? v : 0, 0);
 		}
 		for (int k = 0; k < 25; ++k) { int v = AM::ld_s8(ma + k); maxsc = maxsc > v ? maxsc : v; }
-		int max_ins = (int)((double)(qlen * maxsc + end_bonus - o_ins) / e_ins + 1.); max_ins = max_ins > 1 ? max_ins : 1;
+		int max_ins = bwag_trunc_i32((double)(qlen * maxsc + end_bonus - o_ins) / e_ins + 1.); max_ins = max_ins > 1 ? max_ins : 1;
 		w = w < max_ins ? w : max_ins;
-		int max_del = (int)((double)(qlen * maxsc + end_bonus - o_del) / e_del + 1.); max_del = max_del > 1 ? max_del : 1;
+		int max_del = bwag_trunc_i32((double)(qlen * maxsc + end_bonus - o_del) / e_del + 1.); max_del = max_del > 1 ? max_del : 1;
 		w = w < max_del ? w : max_del;
 	}
 	__syncwarp();

@@ -49,8 +49,8 @@ __device__ __forceinline__ u32 k4l_rc(u32 lo, u32 hi, u32 s) { return __funnelsh
 
 __device__ __forceinline__ int k4l_max_gap(const bwag_sw_par_t &p, int qlen) /* cal_max_gap, bwamem.c:647-654 */
 {
-	int l_del = (int)((double)(qlen * p.a - p.o_del) / p.e_del + 1.);
-	int l_ins = (int)((double)(qlen * p.a - p.o_ins) / p.e_ins + 1.);
+	int l_del = bwag_trunc_i32((double)(qlen * p.a - p.o_del) / p.e_del + 1.);
+	int l_ins = bwag_trunc_i32((double)(qlen * p.a - p.o_ins) / p.e_ins + 1.);
 	int l = l_del > l_ins ? l_del : l_ins;
 	l = l > 1 ? l : 1;
 	return l < p.w << 1 ? l : p.w << 1;
@@ -240,9 +240,9 @@ __global__ void __launch_bounds__(K4L_THREADS, K4L_MINB) k_extend_lane(DevIndex 
 						H1 = h0 > oe_ins ? h0 - oe_ins : 0;
 						qp = phase == 0 ? query + s_qbeg - 1 : query + s_qbeg + s_len;
 						qs = phase == 0 ? -1 : 1;
-						int max_ins = (int)((double)(qlen * maxsc + end_bonus - o_ins) / e_ins + 1.); max_ins = max_ins > 1 ? max_ins : 1;
+						int max_ins = bwag_trunc_i32((double)(qlen * maxsc + end_bonus - o_ins) / e_ins + 1.); max_ins = max_ins > 1 ? max_ins : 1;
 						w = w < max_ins ? w : max_ins;
-						int max_del = (int)((double)(qlen * maxsc + end_bonus - o_del) / e_del + 1.); max_del = max_del > 1 ? max_del : 1;
+						int max_del = bwag_trunc_i32((double)(qlen * maxsc + end_bonus - o_del) / e_del + 1.); max_del = max_del > 1 ? max_del : 1;
 						w = w < max_del ? w : max_del;
 					}
 					mx = h0; max_i = max_j = -1; max_ie = -1; gscore = -1; max_off = 0;

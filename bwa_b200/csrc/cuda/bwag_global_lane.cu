@@ -79,8 +79,8 @@ __global__ void __launch_bounds__(K5L_THREADS, 2) k_global_lane(DevIndex ix, Glb
 				w2 = w2 < p.w << 2 ? w2 : p.w << 2;
 				int max_gap, max_ins, max_del, min_w, d = rlen - lq;
 				d = d < 0 ? -d : d;
-				max_ins = (int)((double)(((lq + 1) >> 1) * s_mat[0] - p.o_ins) / p.e_ins + 1.);
-				max_del = (int)((double)(((lq + 1) >> 1) * s_mat[0] - p.o_del) / p.e_del + 1.);
+				max_ins = bwag_trunc_i32((double)(((lq + 1) >> 1) * s_mat[0] - p.o_ins) / p.e_ins + 1.);
+				max_del = bwag_trunc_i32((double)(((lq + 1) >> 1) * s_mat[0] - p.o_del) / p.e_del + 1.);
 				max_gap = max_ins > max_del ? max_ins : max_del;
 				max_gap = max_gap > 1 ? max_gap : 1;
 				w = (max_gap + d + 1) >> 1;

@@ -292,7 +292,7 @@ static int launch_extend(bwag_batch_t *b, ExtArgs &a, int n_units, int n_many = 
 			ExtArgs la = a;
 			la.eh = 0; la.rseq = 0; la.smem_per_warp = lcols;   /* here: the number of columns of a lane's row */
 			la.chain_lo = 0; la.chain_hi = many;
-			if (getenv("BWA_B200_PROFILE")) fprintf(stderr, "[prof] extension: lane-per-read kernel, grid %d x %d, %zu bytes of shared memory per block\n", lgrid, K4L_THREADS, lsm);
+			if (getenv("BWA_B200_PROFILE")) fprintf(stderr, "[prof] extension: lane-per-read kernel for reads with chains %d..%d, grid %d x %d, %zu bytes of shared memory per block\n", la.chain_lo, la.chain_hi, lgrid, K4L_THREADS, lsm);
 			BWAG_LAUNCH(k_extend_lane, lgrid, K4L_THREADS, lsm, c->stream, c->ix, la);
 			CK(cudaGetLastError());
 			++c->st.n_launch;
@@ -306,6 +306,10 @@ static int launch_extend(bwag_batch_t *b, ExtArgs &a, int n_units, int n_many = 
 #endif
 	i64 need = ((i64)n_units + wpb - 1) / wpb;
 	if (grid > need) grid = (int)(need > 0 ? need : 1);
+	if (getenv("BWA_B200_PROFILE"))
+		fprintf(stderr, "[prof] extension: warp-per-read kernel %s (scratch in %s memory, %s row sweep) for reads with chains %d..%d, grid %d x %d\n",
+		        use_sm ? (fast ? "k_extend_sm_fast" : "k_extend_sm") : (fast ? "k_extend_fast" : "k_extend"), use_sm ? "shared" : "global",
+		        fast ? "lean" : "first", a.chain_lo, a.chain_hi, grid, K4_THREADS);
 	if (!use_sm) {
 		const size_t n_warps = (size_t)grid * wpb;
 		if (buf_reserve(&c->s_eh, n_warps * 2 * (size_t)(a.cap_q + 2) * 4) || buf_reserve(&c->s_rseq, n_warps * (size_t)a.cap_r)) return 1;
@@ -726,6 +730,10 @@ int run_global(bwag_batch_t *b, const bwag_sw_par_t *par, int n_tasks, int cap_q
 			++c->st.n_launch;
 		}
 		a.smem_per_warp = k5_sm ? k5_per_warp : 0; a.z_sm_bytes = k5_sm ? k5_zsm : 0;
+		if (getenv("BWA_B200_PROFILE"))
+			fprintf(stderr, "[prof] global alignment: warp-per-request kernel %s (scratch in %s memory, %s row sweep), %d requests, grid %d x %d\n",
+			        k5_sm ? (k5_fast ? "k_global_sm_fast" : "k_global_sm") : (k5_fast ? "k_global_fast" : "k_global"), k5_sm ? "shared" : "global",
+			        k5_fast ? "lean" : "first", n_tasks, grid, K5_THREADS);
 		if (k5_sm && k5_fast) BWAG_LAUNCH(k_global_sm_fast, grid, K5_THREADS, k5_smem, c->stream, c->ix, a);
 		else if (k5_sm) BWAG_LAUNCH(k_global_sm, grid, K5_THREADS, k5_smem, c->stream, c->ix, a);
 		else if (k5_fast) BWAG_LAUNCH(k_global_fast, grid, K5_THREADS, 0, c->stream, c->ix, a);

@@ -84,7 +84,7 @@ __global__ void __launch_bounds__(SE_THREADS) k_se_refine(DevIndex ix, SeArgs a)
 			qs[x] = c;
 		}
 		__syncwarp();
-		int w = (int)(abs(rlen - len) * 1.5);
+		int w = (int)(abs(rlen - len) * 1.5);   /* in range: rlen - len is the hit's n_del - n_ins */
 		w = SE_BAND > w ? SE_BAND : w;
 		const int n_col = len < 2 * w + 1 ? len : 2 * w + 1;
 		warp_ksw_global(lane, len, qs, rlen, rs, s_mat, 5, 1, 5, 1, w, H, E, z, n_col, &cells);
@@ -244,7 +244,7 @@ int se_list_read(SeList &L, const bwag_se_read_t &p, const bwag_se_hit_t *multi,
 		if (k < 0 ? !gapped : !multi[slot].gap) continue;
 		const int rlen = p.len + (k < 0 ? p.ref_shift : multi[slot].ref_shift);
 		if (rlen < 0) return set_err("read %d of the batch: a gapped hit with %d reference bases", r, rlen);
-		int w = (int)(abs(rlen - p.len) * 1.5);
+		int w = (int)(abs(rlen - p.len) * 1.5);   /* in range: rlen - len is the hit's n_del - n_ins */
 		w = w > 50 ? w : 50;
 		const i64 n_col = p.len < 2 * w + 1 ? p.len : 2 * w + 1;
 		mt = L.n_tasks;

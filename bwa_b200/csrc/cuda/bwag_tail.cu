@@ -59,7 +59,7 @@ __device__ __forceinline__ int t_infer_bw(int l1, int l2, int score, int a, int 
 {
 	int w;
 	if (l1 == l2 && l1 * a - score < (q + r - a) << 1) return 0;
-	w = (int)(((double)((l1 < l2 ? l1 : l2) * a - score - q) / r + 2.));
+	w = bwag_trunc_i32(((double)((l1 < l2 ? l1 : l2) * a - score - q) / r + 2.));
 	const int d = l1 > l2 ? l1 - l2 : l2 - l1;
 	if (w < d) w = d;
 	return w;
@@ -295,16 +295,16 @@ __device__ int t_mapq_se(const mem_opt_t &opt, const mem_alnreg_t &a, const doub
 		if (l >= TAIL_LOGN) { *cx = BWAG_CX_LONG; return 0; }
 		tmp = l < opt.mapQ_coef_len ? 1. : opt.mapQ_coef_fac / logtab[l];
 		tmp *= identity * identity;
-		mapq = (int)(6.02 * (a.score - sub) / opt.a * tmp * tmp + .499);
+		mapq = bwag_trunc_i32(6.02 * (a.score - sub) / opt.a * tmp * tmp + .499);
 	} else {
 		if (a.seedcov < 0 || a.seedcov >= TAIL_LOGN) { *cx = BWAG_CX_LONG; return 0; }
-		mapq = (int)(30.0 * (1. - (double)sub / a.score) * logtab[a.seedcov] + .499);
-		mapq = identity < 0.95 ? (int)(mapq * identity * identity + .499) : mapq;
+		mapq = bwag_trunc_i32(30.0 * (1. - (double)sub / a.score) * logtab[a.seedcov] + .499);
+		mapq = identity < 0.95 ? bwag_trunc_i32(mapq * identity * identity + .499) : mapq;
 	}
-	if (a.sub_n > 0) mapq -= (int)(4.343 * logtab[a.sub_n + 1] + .499);
+	if (a.sub_n > 0) mapq -= bwag_trunc_i32(4.343 * logtab[a.sub_n + 1] + .499);
 	if (mapq > 60) mapq = 60;
 	if (mapq < 0) mapq = 0;
-	mapq = (int)(mapq * (1. - a.frac_rep) + .499);
+	mapq = bwag_trunc_i32(mapq * (1. - a.frac_rep) + .499);
 	return mapq;
 }
 
@@ -380,7 +380,7 @@ __device__ int t_pair(const TailSamArgs &g, const mem_alnreg_t *a0, int n0, cons
 				if (dist > g.pes[dir].high) break;
 				if (dist < g.pes[dir].low) continue;
 				if (!g.ptab[dir]) return -1;
-				int q = (int)((v[i].y >> 32) + (v[k].y >> 32) + g.ptab[dir][dist - g.pes[dir].low] + .499);
+				int q = bwag_trunc_i32((v[i].y >> 32) + (v[k].y >> 32) + g.ptab[dir][dist - g.pes[dir].low] + .499);
 				if (q < 0) q = 0;
 				if (nu == 16) return -1;
 				P64 p;
@@ -620,11 +620,11 @@ __global__ void __launch_bounds__(128) k_tail_sam(TailSamArgs g)
 			int q_pe, q_se[2];
 			const int score_un = regs[0][0].score + regs[1][0].score - opt.pen_unpaired;
 			subo = subo > score_un ? subo : score_un;
-			q_pe = (int)(6.02 * (o - subo) / opt.a + .499);
-			if (n_sub > 0) { if (n_sub + 1 >= TAIL_LOGN) cx = BWAG_CX_PAIR; else q_pe -= (int)(4.343 * g.logtab[n_sub + 1] + .499); }
+			q_pe = bwag_trunc_i32(6.02 * (o - subo) / opt.a + .499);
+			if (n_sub > 0) { if (n_sub + 1 >= TAIL_LOGN) cx = BWAG_CX_PAIR; else q_pe -= bwag_trunc_i32(4.343 * g.logtab[n_sub + 1] + .499); }
 			if (q_pe < 0) q_pe = 0;
 			if (q_pe > 60) q_pe = 60;
-			q_pe = (int)(q_pe * (1. - .5 * (regs[0][0].frac_rep + regs[1][0].frac_rep)) + .499);
+			q_pe = bwag_trunc_i32(q_pe * (1. - .5 * (regs[0][0].frac_rep + regs[1][0].frac_rep)) + .499);
 			if (o > score_un) {
 				mem_alnreg_t *c[2] = { &regs[0][z[0]], &regs[1][z[1]] };
 				for (int i = 0; i < 2; ++i) {
@@ -635,7 +635,7 @@ __global__ void __launch_bounds__(128) k_tail_sam(TailSamArgs g)
 				q_se[1] = q_se[1] > q_pe ? q_se[1] : q_pe < q_se[1] + 40 ? q_pe : q_se[1] + 40;
 				extra_flag |= 2;
 				for (int i = 0; i < 2; ++i) {
-					const int cap = (int)(6.02 * (c[i]->score - c[i]->csub) / opt.a + .499);
+					const int cap = bwag_trunc_i32(6.02 * (c[i]->score - c[i]->csub) / opt.a + .499);
 					q_se[i] = q_se[i] < cap ? q_se[i] : cap;
 				}
 			} else {

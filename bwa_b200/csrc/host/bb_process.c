@@ -20,6 +20,7 @@
 #include <assert.h>
 #include <math.h>
 #include <malloc.h>
+#include <unistd.h>
 #include "bb_host.h"
 #if defined(__SSE2__)
 #include <emmintrin.h>
@@ -572,6 +573,33 @@ static void w_dedup(void *d, long i, int tid)
 	r->dedup_done = 1;
 }
 
+/* Test hook: BWA_B200_TEST_DUMP_STAGES=<dir> writes the inputs of every bwag_extend and bwag_global call to a file of its own in
+ * <dir>, so that tests/test_dp_stages.py can replay them through two implementations of the stage ABI.  Every file is in the host's
+ * byte order: eight int64 (kind 1 = extend, 2 = global; n_reads; bases; n_chains or n_tasks; n_seeds; and the sizes of
+ * bwag_sw_par_t and of a chain or task), the bwag_sw_par_t, off[n_reads + 1], the bases (codes 0..4), then for an extension
+ * chain_off[n_reads + 1], the chains and the seeds, for a global alignment the tasks. */
+static void dump_stage(const job_t *j, const bwag_sw_par_t *swp, int kind, int64_t n_items, const void *items, size_t item_size)
+{
+	static int seq;
+	const char *dir = getenv("BWA_B200_TEST_DUMP_STAGES");
+	char path[4096];
+	FILE *fp;
+	if (!dir) return;
+	snprintf(path, sizeof(path), "%s/%s-%d-%06d.bin", dir, kind == 1 ? "extend" : "global", (int)getpid(), __atomic_fetch_add(&seq, 1, __ATOMIC_RELAXED));
+	if (!(fp = fopen(path, "wb"))) bb_fatal("mem_process_seqs", "cannot write %s", path);
+	{
+		const int64_t h[8] = { kind, j->n, j->off[j->n], n_items, kind == 1 ? j->n_xseeds : 0, (int64_t)sizeof(*swp), (int64_t)item_size, 0 };
+		fwrite(h, sizeof(h), 1, fp);
+	}
+	fwrite(swp, sizeof(*swp), 1, fp);
+	fwrite(j->off, sizeof(int64_t), (size_t)j->n + 1, fp);
+	fwrite(j->codes, 1, (size_t)j->off[j->n], fp);
+	if (kind == 1) fwrite(j->chain_off, sizeof(int32_t), (size_t)j->n + 1, fp);
+	fwrite(items, item_size, (size_t)n_items, fp);
+	if (kind == 1) fwrite(j->xseeds, sizeof(bwag_xseed_t), (size_t)j->n_xseeds, fp);
+	if (fclose(fp) != 0) bb_fatal("mem_process_seqs", "cannot write %s", path);
+}
+
 /* serve every outstanding alignment request of the batch with one device call; returns #requests */
 typedef struct { job_t *j; int64_t *off; bwag_gtask_t *tasks; const bwag_galn_t *out; int64_t *boff; char *block; } ground_t;
 
@@ -639,6 +667,7 @@ static int64_t global_round(job_t *j, bwag_batch_t *batch, const bwag_sw_par_t *
 	if (t == 0) { big_free(g.off); return 0; }
 	g.tasks = big_alloc_x(sizeof(bwag_gtask_t) * (size_t)t, 1);
 	bb_parallel_for_lane(j->lane, nt, w_gfill, &g, j->n);
+	dump_stage(j, swp, 2, t, g.tasks, sizeof(bwag_gtask_t));
 	if (bwag_global(batch, swp, (int)t, g.tasks, &out) != 0) bb_fatal("mem_process_seqs", "global-alignment stage failed: %s", bwag_last_error());
 	g.boff = big_alloc(sizeof(int64_t) * ((size_t)t + 1));
 	{
@@ -838,6 +867,7 @@ static void host_chain_extend(job_t *j, bwag_batch_t *batch, const bwag_sw_par_t
 	big_free(j->slice); j->slice = 0;
 	PH(j, "flatten");
 
+	dump_stage(j, swp, 1, nc, j->xchains, sizeof(bwag_xchain_t));
 	if (bwag_extend(batch, swp, j->chain_off, j->xchains, j->n_xseeds, j->xseeds, &j->xregs) != 0)
 		bb_fatal("mem_process_seqs", "extension stage failed: %s", bwag_last_error());
 	PH(j, "extend_stage");
